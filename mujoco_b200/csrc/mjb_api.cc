@@ -160,6 +160,7 @@ mjbBatch* mjb_make_batch(const struct mjModel_* m, int nenv, int nconmax, int nj
   b.nlane = (H.sz.nbody <= 16 && H.sz.nv <= 16 && H.opt.solver != SOL_PGS) ? 16 : 32;
   b.xfrc = 0;
   if (const char* ls = getenv("MJB_LANES")) { const int v = atoi(ls); if (v == 16 || v == 32) b.nlane = v; }
+  if (H.sz.convex) b.nlane = 32;   // the convex narrow phase is built for the 32-lane mapping only
   b.dpitch = ((size_t)b.L.ndbl + 15) / 16 * 16;   // env-major blocks, 128-byte aligned
   b.ipitch = ((size_t)b.L.nint + 31) / 32 * 32;
   size_t nd = b.dpitch * b.stride;

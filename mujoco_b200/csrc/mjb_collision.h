@@ -664,6 +664,13 @@ MJB_HD int collide_box_box(PreCon* c, double margin, V3 p1, const M3& m1, const 
   return naccept;
 }
 
+}  // namespace mjb
+
+// convex narrow phase (GJK / EPA, plane-ellipsoid), only in kernels compiled with FEAT_CONVEX
+#include "mjb_convex.h"
+
+namespace mjb {
+
 // filter + narrowphase of candidate pair p; returns the number of pre-contacts written to pc[]
 MJB_HD int pair_collide(const Env& d, int p, PreCon* pc) {
   const DModel& m = d.m;
@@ -703,10 +710,90 @@ MJB_HD int pair_collide(const Env& d, int p, PreCon* pc) {
   return 0;
 }
 
+// ordinal of GJK candidate p among the GJK candidates of the table (its entry in the pre-contact store ccd_con)
+MJB_HD int gjk_ordinal(const DModel& m, int p) {
+  int c = 0;
+  for (int q = 0; q < p; q++) c += pair_gjk(m.geom_type[m.pair_geom1[q]], m.geom_type[m.pair_geom2[q]]) ? 1 : 0;
+  return c;
+}
+
+// GJK / EPA candidates, before the count pass: the first K lanes of the environment each take every K-th GJK candidate
+// in table order, with their own polytope slot (K = the environment's slots, at most its lanes), and store the
+// candidate's pre-contacts, so that neither pass of collision_t evaluates it again
+MJB_HD void convex_pass(const Env& d) {
+  const DModel& m = d.m;
+  const int npair = m.sz.npair;
+  int K = kCcdSlots < d.nlane ? kCcdSlots : d.nlane;
+  if (m.sz.ccdslots < K) K = m.sz.ccdslots;
+  if (d.lane < K) {
+    double* slot = &d.ccd_poly()[(long)d.lane * m.sz.ccdslot];
+    FD store = d.ccd_con();
+    FD gx = d.geom_xpos(), gm = d.geom_xmat();
+    int c = 0;
+    for (int p = 0; p < npair; p++) {
+      const int g1 = m.pair_geom1[p], g2 = m.pair_geom2[p];
+      if (!pair_gjk(m.geom_type[g1], m.geom_type[g2])) continue;
+      if (c++ % K != d.lane) continue;
+      const long base = 36L * (c - 1);
+      const double margin = m.pair_margin[p];
+      const V3 p1 = ld3(gx, 3 * g1), p2 = ld3(gx, 3 * g2);
+      const V3 dif = p1 - p2;   // bounding-sphere filter (mj_filterSphere); neither geom is a plane
+      const double dsq = dif.x * dif.x + dif.y * dif.y + dif.z * dif.z;
+      const double bound = m.geom_rbound[g1] + m.geom_rbound[g2] + margin;
+      int n = 0;
+      PreCon pc[5];
+      if (!(dsq > bound * bound)) n = collide_convex(pc, m, g1, g2, p1, ld9(gm, 9 * g1), p2, ld9(gm, 9 * g2), margin, slot);
+      store[base] = n;
+      for (int k = 0; k < n; k++) {
+        const long o = base + 1 + 7 * k;
+        store[o] = pc[k].dist;
+        st3(store, o + 1, pc[k].pos);
+        st3(store, o + 4, pc[k].normal);
+      }
+    }
+  }
+  MJB_PSYNC();
+}
+
+// pre-contacts of GJK candidate p stored by convex_pass; returns their number
+MJB_HD int convex_load(const Env& d, int p, PreCon* pc);
+
+// candidate p in a FEAT_CONVEX kernel: GJK candidates from the store of convex_pass, plane-ellipsoid (after the plane
+// filter of mj_filterSphere), every other pair through pair_collide
+MJB_HD int pair_collide_convex(const Env& d, int p, PreCon* pc) {
+  const DModel& m = d.m;
+  const int g1 = m.pair_geom1[p], g2 = m.pair_geom2[p];
+  const int t1 = m.geom_type[g1], t2 = m.geom_type[g2];
+  if (pair_gjk(t1, t2)) return convex_load(d, p, pc);
+  if (t1 != GEOM_PLANE || t2 != GEOM_ELLIPSOID) return pair_collide(d, p, pc);
+  FD gx = d.geom_xpos(), gm = d.geom_xmat();
+  const double margin = m.pair_margin[p];
+  const V3 p1 = ld3(gx, 3 * g1), p2 = ld3(gx, 3 * g2);
+  if (m.geom_rbound[g2] > 0) {
+    const V3 nrm{gm[9 * g1 + 2], gm[9 * g1 + 5], gm[9 * g1 + 8]};
+    if (dot(p2 - p1, nrm) > margin + m.geom_rbound[g2]) return 0;
+  }
+  return collide_plane_ellipsoid(pc[0], margin, p1, ld9(gm, 9 * g1), p2, ld9(gm, 9 * g2), m.geom_size + 3 * g2);
+}
+
+MJB_HD int convex_load(const Env& d, int p, PreCon* pc) {
+  FD store = d.ccd_con();
+  const long base = 36L * gjk_ordinal(d.m, p);
+  const int n = (int)store[base];
+  for (int k = 0; k < n; k++) {
+    const long o = base + 1 + 7 * k;
+    pc[k].dist = store[o];
+    pc[k].pos = ld3(store, o + 1);
+    pc[k].normal = ld3(store, o + 4);
+    pc[k].tangent = V3{0, 0, 0};
+  }
+  return n;
+}
+
 // walk the static candidate table cooperatively in two passes: (1) every lane counts the
 // pre-contacts of its candidates, (2) after a serial scan that assigns contact slots IN TABLE ORDER
 // (the reference's emission order) the few hitting pairs are evaluated again and written in place.
-template <int MAXC>
+template <int MAXC, bool CONVEX = false>
 MJB_HD void collision_t(const Env& d) {
   const DModel& m = d.m;
   FI ncon_f = d.ncon();
@@ -717,9 +804,11 @@ MJB_HD void collision_t(const Env& d) {
   }
   FI cnt = d.scr_ipair();        // per pair: number of pre-contacts, then packed (offset | n << 24)
   const int npair = m.sz.npair, nconmax = m.sz.nconmax;
+  if constexpr (CONVEX) convex_pass(d);
   MJB_PFOR(p, npair) {
     PreCon pc[MAXC];
-    cnt[p] = pair_collide(d, p, pc);
+    if constexpr (CONVEX) cnt[p] = pair_collide_convex(d, p, pc);
+    else cnt[p] = pair_collide(d, p, pc);
   }
   MJB_PSYNC();
   MJB_LANE0 {   // exclusive scan in table order, capped at nconmax
@@ -743,7 +832,8 @@ MJB_HD void collision_t(const Env& d) {
     const int off = cnt[p] & 0xFFFFFF, n = cnt[p] >> 24;
     if (!n) continue;
     PreCon pc[MAXC];
-    pair_collide(d, p, pc);
+    if constexpr (CONVEX) pair_collide_convex(d, p, pc);
+    else pair_collide(d, p, pc);
     for (int k = 0; k < n; k++) {
       const int c = off + k;
       const double dist = pc[k].dist;
@@ -772,8 +862,16 @@ MJB_HD void collision_t(const Env& d) {
 }
 
 // pairs of the sphere / capsule / plane family give at most two contacts; the cylinder and box colliders up to
-// eight (kernels without FEAT_COLBOX do not carry their code or the larger pre-contact array)
+// eight, the convex pairs up to five (kernels without FEAT_COLBOX / FEAT_CONVEX do not carry their code or the larger
+// pre-contact array)
+// On the device the convex branch is compiled only in the translation unit that defines MJB_CONVEX_UNIT (the
+// FEAT_CONVEX instantiations, mjb_kstep_convex32.cu): in every other kernel collision() is the same code as without the
+// convex narrow phase, so their inlining and stack layout do not see GJK / EPA at all.  Host compilations (the
+// emulation of the device path) always carry it.
 MJB_HD void collision(const Env& d) {
+#if defined(MJB_CONVEX_UNIT) || !defined(__CUDA_ARCH__)
+  if (d.feat & FEAT_CONVEX) { collision_t<8, true>(d); return; }
+#endif
   if (d.feat & FEAT_COLBOX) collision_t<8>(d); else collision_t<2>(d);
 }
 

@@ -204,17 +204,23 @@ int launch_fill_zero(const Batch& b, int is_int, long off, long cnt, void* s) {
   return 0;
 }
 
+// lean kernels (FEAT = 0) when the model needs none of the optional pipeline parts (FEAT_*); a model with convex
+// collision pairs is never lean, since only the FEAT_CONVEX instantiations carry its narrow phase
+static bool lean_model(const DModel& dm, const Batch& b) {
+  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc && !dm.sz.convex;
+}
+
 // split step: position + velocity | PGS (4 lanes per environment, mjb_pgs4.cu) | finish + integrate | redo
 // launch for environments whose acceleration check failed (exits at once everywhere else).
 bool split_step_available(const DModel& dm, const Batch& b) {
   static int want = -1;
   if (want < 0) { const char* s = getenv("MJB_SPLIT"); want = s ? atoi(s) : 1; }
   const bool islands = dm.sz.ntree > 1 && !(dm.opt.disableflags & DSBL_ISLAND);
-  return want && b.warp_per_env && b.nlane == 32 && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
+  return want && b.warp_per_env && b.nlane == 32 && !dm.sz.convex && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
          (dm.opt.integrator == INT_EULER || dm.opt.integrator == INT_IMPLICITFAST);
 }
 int launch_split_step(const DModel& dm, const Batch& b, int first, int later, void* s, void* stagger) {
-  const bool lean = dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc;
+  const bool lean = lean_model(dm, b);
   static const int part_lanes = [] { const char* e = getenv("MJB_PART_LANES"); return e ? atoi(e) : 16; }();
   if (lean && part_lanes == 16) launch_kpart1_lean16(dm, b, 0, first, s);
   else if (lean && part_lanes == 8) launch_kpart1_lean8(dm, b, 0, first, s);
@@ -240,9 +246,6 @@ int launch_split_step(const DModel& dm, const Batch& b, int first, int later, vo
 // of a step - gains more than the halves of the step lose to the PGS pool's share of L1.  Bit-identical to the split
 // step, which the tests compare it with.
 static int g_persistent = -1;
-static bool lean_model(const DModel& dm, const Batch& b) {
-  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc;
-}
 bool rollout_persistent_available(const DModel& dm, const Batch& b, int nstep) {
   if (g_persistent < 0) { const char* e = getenv("MJB_PERSISTENT"); g_persistent = e ? atoi(e) : 1; }
   static const int part_lanes = [] { const char* e = getenv("MJB_PART_LANES"); return e ? atoi(e) : 16; }();
@@ -268,7 +271,7 @@ int profile_split_step(const DModel& dm, const Batch& b, void* s, float* ms) {
   cudaStream_t st = (cudaStream_t)s;
   cudaEvent_t ev[5];
   for (auto& e : ev) CK(cudaEventCreate(&e), "event create");
-  const bool lean = dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc;
+  const bool lean = lean_model(dm, b);
   static const int part_lanes = [] { const char* e = getenv("MJB_PART_LANES"); return e ? atoi(e) : 16; }();
   cudaEventRecord(ev[0], st);
   if (lean && part_lanes == 16) launch_kpart1_lean16(dm, b, 0, 1, s);
@@ -293,9 +296,11 @@ int profile_split_step(const DModel& dm, const Batch& b, void* s, float* ms) {
 }
 
 int launch_stages(const DModel& dm, const Batch& b, int mask, int flags, void* s) {
-  if (b.warp_per_env) {
+  if (dm.sz.convex) {   // convex collision pairs: only these instantiations carry GJK / EPA (32 lanes or one lane per env)
+    if (b.warp_per_env) launch_kstep_convex32(dm, b, mask, flags, s); else launch_kstep_lane_convex(dm, b, mask, flags, s);
+  } else if (b.warp_per_env) {
     // lean kernels when the model needs none of the optional pipeline parts (FEAT_*)
-    const bool lean = dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc;
+    const bool lean = lean_model(dm, b);
     if (b.nlane == 16) {
       if (dm.opt.solver == SOL_NEWTON) { if (lean) launch_kstep_newton16_lean(dm, b, mask, flags, s); else launch_kstep_newton16(dm, b, mask, flags, s); }
       else launch_kstep_any16(dm, b, mask, flags, s);

@@ -12,6 +12,7 @@
 //   src/engine/engine_core_util.c:1119-1215  mj_actuatorDamping / mj_actuatorArmature
 //   src/engine/engine_forward.c:1409-1421    which dofs trigger implicit Euler damping
 #include "mjb_model.h"
+#include "mjb_collision.h"   // pair_gjk, kCcdSlots, ccd_slot_doubles (convex candidates and their scratch)
 
 #include <algorithm>
 #include <cstdio>
@@ -212,11 +213,16 @@ static bool collider_boxfamily(int t1, int t2) {  // t1 <= t2
   return is(mjGEOM_PLANE, mjGEOM_CYLINDER) || is(mjGEOM_PLANE, mjGEOM_BOX) || is(mjGEOM_SPHERE, mjGEOM_CYLINDER) ||
          is(mjGEOM_SPHERE, mjGEOM_BOX) || is(mjGEOM_CAPSULE, mjGEOM_BOX) || is(mjGEOM_BOX, mjGEOM_BOX);
 }
+// convex narrow phase (mjb_convex.h, compiled into the FEAT_CONVEX kernels): plane-ellipsoid (mjc_PlaneConvex) and the
+// primitive pairs the reference sends to mjc_Convex (GJK / EPA, up to five contacts per pair with multiCCD)
+static bool collider_convex(int t1, int t2) {  // t1 <= t2
+  return (t1 == mjGEOM_PLANE && t2 == mjGEOM_ELLIPSOID) || pair_gjk(t1, t2);
+}
 static bool collider_supported(int t1, int t2) {  // t1 <= t2
   auto is = [&](int a, int b) { return t1 == a && t2 == b; };
   return is(mjGEOM_PLANE, mjGEOM_SPHERE) || is(mjGEOM_PLANE, mjGEOM_CAPSULE) ||
          is(mjGEOM_SPHERE, mjGEOM_SPHERE) || is(mjGEOM_SPHERE, mjGEOM_CAPSULE) ||
-         is(mjGEOM_CAPSULE, mjGEOM_CAPSULE) || collider_boxfamily(t1, t2);
+         is(mjGEOM_CAPSULE, mjGEOM_CAPSULE) || collider_boxfamily(t1, t2) || collider_convex(t1, t2);
 }
 static bool collider_defined(int t1, int t2) {  // mjCOLLISIONFUNC != NULL, t1 <= t2
   if (t1 == mjGEOM_PLANE) return t2 != mjGEOM_PLANE && t2 != mjGEOM_HFIELD;
@@ -434,7 +440,7 @@ int check_model(const mjModel* m) {
     int t = m->geom_type[i];
     if (t == mjGEOM_HFIELD || t == mjGEOM_SDF) FAIL("geom %d: hfield/sdf", i);
     if (m->geom_contype[i] == 0 && m->geom_conaffinity[i] == 0) continue;
-    if (t == mjGEOM_MESH || t == mjGEOM_ELLIPSOID) FAIL("geom %d: mesh/ellipsoid colliders are a 'next' row", i);
+    if (t == mjGEOM_MESH) FAIL("geom %d: mesh colliders are a 'next' row", i);
   }
 #undef FAIL
   return 0;
@@ -483,6 +489,8 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
   for (int i = 0; i < m->nu; i++) if (m->actuator_trntype[i] == mjTRN_SITE || m->actuator_trntype[i] == mjTRN_SLIDERCRANK) S.sitetrn = 1;
   S.gravcomp = m->flg_gravcomp ? 1 : 0;
   S.colbox = 0;   // set while the candidate pairs are built
+  S.convex = 0;
+  S.nconvex = 0;
   S.freebody = 0;
   if (m->opt.integrator == mjINT_IMPLICITFAST)
     for (int j = 0; j < m->njnt; j++) {
@@ -515,6 +523,7 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
   O.density = m->opt.density; O.viscosity = m->opt.viscosity;
   for (int i = 0; i < 3; i++) O.wind[i] = m->opt.wind[i];
   O.meaninertia = m->stat.meaninertia;
+  O.ccd_iterations = m->opt.ccd_iterations; O.ccd_tolerance = m->opt.ccd_tolerance;
   O.integrator = m->opt.integrator; O.cone = m->opt.cone; O.solver = m->opt.solver;
   O.iterations = m->opt.iterations; O.ls_iterations = m->opt.ls_iterations;
   O.noslip_iterations = m->opt.noslip_iterations; O.noslip_tolerance = m->opt.noslip_tolerance;
@@ -820,6 +829,24 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
   // a pair is tested before the first body pair whose signature is not smaller, the rest after the walk - with the
   // pair's own parameters and none of the body / bitmask filters
   int pairadr = 0;
+  // convex candidates: the libccd path that mjDSBL_NATIVECCD selects for the GJK pairs is not built (plane-ellipsoid
+  // never uses it), and ccd_iterations sizes the EPA polytope, whose faces name their vertices in 10 bits
+  auto note_convex = [&](int t1, int t2) -> int {
+    if (!collider_convex(t1, t2)) return 0;
+    if (pair_gjk(t1, t2)) {
+      if (m->opt.disableflags & mjDSBL_NATIVECCD) {
+        set_error("unsupported: mjDSBL_NATIVECCD (the libccd convex collision path) is not built; only native GJK / EPA is");
+        return -2;
+      }
+      if (m->opt.ccd_iterations < 1 || m->opt.ccd_iterations > 1000) {
+        set_error("unsupported: ccd_iterations outside [1, 1000] with convex collision pairs");
+        return -2;
+      }
+      S.nconvex++;
+    }
+    S.convex = 1;
+    return 0;
+  };
   auto push_predefined = [&](int k) -> int {
     int x = m->pair_geom1[k], y = m->pair_geom2[k];
     if (m->geom_type[x] > m->geom_type[y]) std::swap(x, y);
@@ -831,6 +858,7 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
       return -2;
     }
     if (collider_boxfamily(m->geom_type[x], m->geom_type[y])) S.colbox = 1;
+    if (int rc = note_convex(m->geom_type[x], m->geom_type[y])) return rc;
     pg1.push_back(x); pg2.push_back(y); pdim.push_back(m->pair_dim[k]);
     pmargin.push_back(m->pair_margin[k] + m->pair_gap[k]); pinc.push_back(m->pair_margin[k]);
     for (int c = 0; c < mjNREF; c++) psolref.push_back(m->pair_solref[mjNREF * k + c]);
@@ -899,6 +927,7 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
           return -2;
         }
         if (collider_boxfamily(m->geom_type[c.g1], m->geom_type[c.g2])) S.colbox = 1;
+        if (int rc = note_convex(m->geom_type[c.g1], m->geom_type[c.g2])) return rc;
         int condim; double solref[mjNREF], solimp[mjNIMP], fr[5];
         contact_param(m, c.g1, c.g2, &condim, solref, solimp, fr);
         double margin = m->geom_margin[c.g1] + m->geom_margin[c.g2];
@@ -926,6 +955,10 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
     }
   }
   S.npair = (int)pg1.size();
+  // polytope scratch of the GJK candidates (mjb_convex.h): kCcdSlots slots per environment, fewer when the model has
+  // fewer GJK candidates; nothing at all for models without them, whose layout is unchanged
+  S.ccdslots = std::min(kCcdSlots, S.nconvex);
+  S.ccdslot = S.nconvex ? (int)ccd_slot_doubles(m->opt.ccd_iterations) : 0;
   B.addI(&D.pair_geom1, pg1.data(), pg1.size());
   B.addI(&D.pair_geom2, pg2.data(), pg2.size());
   B.addI(&D.pair_dim, pdim.data(), pdim.size());

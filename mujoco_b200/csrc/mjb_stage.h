@@ -98,6 +98,12 @@ MJB_HD void run_env(const DModel& m, const Batch& b, int e, int mask, int flags,
                     double* sm, int smcap, int solver = -1, unsigned lanes = 0xffffffffu, int feat = FEAT_ALL,
                     int part = 0) {
   Env d(m, b, e, lane, nlane);
+#if !defined(__CUDA_ARCH__)
+  // a host compilation of this code (the emulation of the device path) is one build for every model: a model with
+  // convex collision pairs takes the convex narrow phase there too.  Device kernels fix their features per
+  // instantiation instead (FEAT_CONVEX only in mjb_kstep_convex32.cu).
+  if (m.sz.convex) feat |= FEAT_CONVEX;
+#endif
   d.sm = sm; d.smcap = smcap; d.mask = lanes; d.feat = feat;
   d.solver = solver < 0 ? m.opt.solver : solver;
   if (flags & 16) {

@@ -31,7 +31,10 @@ enum { STATE_SATISFIED = 0, STATE_QUADRATIC = 1, STATE_LINEARNEG = 2, STATE_LINE
 enum { WARN_INERTIA = 0, WARN_CONTACTFULL = 1, WARN_CNSTRFULL = 2, WARN_BADQPOS = 3,
        WARN_BADQVEL = 4, WARN_BADQACC = 5, WARN_BADCTRL = 6, WARN_VGEOMFULL = 7, NWARNING = 8 };
 enum { NISLAND = 20 };
-enum { FEAT_SENSOR = 1, FEAT_EQUALITY = 2, FEAT_ISLAND = 4, FEAT_IMPLICITFAST = 8, FEAT_ACT = 16, FEAT_COLBOX = 32, FEAT_ALL = 63 };   // FEAT_COLBOX: cylinder / box colliders (up to 8 contacts per pair)   // FEAT_ACT: stateful actuators (act), tendon transmissions, muscles
+enum { FEAT_SENSOR = 1, FEAT_EQUALITY = 2, FEAT_ISLAND = 4, FEAT_IMPLICITFAST = 8, FEAT_ACT = 16, FEAT_COLBOX = 32, FEAT_ALL = 63,
+       FEAT_CONVEX = 64 };   // FEAT_COLBOX: cylinder / box colliders (up to 8 contacts per pair)   // FEAT_ACT: stateful actuators (act), tendon transmissions, muscles
+// FEAT_CONVEX: GJK / EPA narrow phase (mjb_convex.h).  Outside FEAT_ALL on purpose: only the convex instantiations
+// carry its code and its polytope scratch, every other kernel compiles exactly as without it.
 enum { EQ_JOINT = 0, EQ_TENDON = 1, EQ_CONNECT = 2, EQ_WELD = 3 };   // supported equality kinds (body semantics)
 constexpr int kNEqData = 11;            // eq_data values per equality (mjNEQDATA): polycoef / anchors, relpose, torquescale
 // sensors of the path (engine_sensor.c); internal codes, translated from mjtSensor by the host
@@ -54,7 +57,8 @@ enum { DSBL_CONSTRAINT = 1 << 0, DSBL_EQUALITY = 1 << 1, DSBL_FRICTIONLOSS = 1 <
        DSBL_CONTACT = 1 << 4, DSBL_SPRING = 1 << 5, DSBL_DAMPER = 1 << 6, DSBL_GRAVITY = 1 << 7,
        DSBL_CLAMPCTRL = 1 << 8, DSBL_WARMSTART = 1 << 9, DSBL_FILTERPARENT = 1 << 10,
        DSBL_ACTUATION = 1 << 11, DSBL_REFSAFE = 1 << 12, DSBL_EULERDAMP = 1 << 15,
-       DSBL_AUTORESET = 1 << 16, DSBL_ISLAND = 1 << 18, DSBL_SENSOR = 1 << 13 };
+       DSBL_AUTORESET = 1 << 16, DSBL_NATIVECCD = 1 << 17, DSBL_ISLAND = 1 << 18, DSBL_SENSOR = 1 << 13,
+       DSBL_MULTICCD = 1 << 19 };
 enum { ENBL_ENERGY = 1 << 1 };   // mjENBL_ENERGY (mjmodel.h mjtEnableBit)                                // :54-73
 enum { LIM_HINGE = 0, LIM_BALL = 1, LIM_TENDON = 2 };   // kinds of limit candidates (host-built table)
 constexpr int kNPoly = 2;   // mjNPOLY (include/mujoco/mjmodel.h:44)
@@ -81,6 +85,10 @@ struct Sizes {
   int ndlevel;   // depth levels of the dof tree
   int nlim;      // limit candidates (joint sides, ball joints, tendon sides) in row order
   int nfl;       // dofs, then tendons, with frictionloss, in row order (fl_dof: dof index, or -(tendon+1))
+  int convex;    // 1 when a candidate pair needs the convex narrow phase (FEAT_CONVEX code paths, mjb_convex.h)
+  int nconvex;   // candidate pairs that go through GJK / EPA (entries of the pre-contact store ccd_con)
+  int ccdslots;  // polytope slots per environment (ccd_poly), 0 without GJK candidates
+  int ccdslot;   // doubles per polytope slot (ccd_slot_doubles(ccd_iterations))
 };
 
 struct Options {
@@ -93,6 +101,8 @@ struct Options {
   int eulerdamp;        // any dof takes the implicit-damping branch of mj_EulerSkip
   int has_limits;       // any limited joint or tendon
   int has_frictionloss; // any dof/tendon frictionloss
+  int ccd_iterations;   // convex narrow phase: GJK / EPA iteration cap, also sizes the EPA polytope
+  double ccd_tolerance; // convex narrow phase: GJK / EPA tolerance
 };
 
 // model arrays: one int blob and one double blob in device memory; members are pointers into them.
@@ -181,6 +191,12 @@ struct DModel {
   X(efc_J, S.njmax * S.nv) X(efc_Y, S.njmax * S.nv) X(efc_AR, S.njmax * S.njmax)                 \
   X(nwt_L, S.nv * S.nv)
 
+// COLD doubles of the convex narrow phase (empty for models without GJK candidates): polytope slots and the stored
+// pre-contacts of the GJK candidates.  Laid out after the other cold fields but declared last in Layout, so that the
+// offsets of every other field stay where they are.
+#define MJB_DATA_CCD_FIELDS(X, S)                                                            \
+  X(ccd_poly, S.ccdslots * S.ccdslot) X(ccd_con, 36 * S.nconvex)
+
 // ints (all hot)
 #define MJB_DATA_INT_FIELDS(X, S)                                                            \
   X(ncon, 1) X(nefc, 1) X(ne, 1) X(nf, 1) X(nl, 1) X(solver_niter, NISLAND) X(step_skip, 1) X(warning, NWARNING)  \
@@ -199,6 +215,9 @@ struct Layout {
 #undef X
   long nhot;         // hot doubles per environment (offsets [0, nhot))
   long ndbl, nint;   // total doubles / ints per environment
+#define X(name, cnt) long name;
+  MJB_DATA_CCD_FIELDS(X, _)
+#undef X
 };
 
 inline Layout make_layout(const Sizes& S) {
@@ -209,6 +228,7 @@ inline Layout make_layout(const Sizes& S) {
   o = (o + 15) / 16 * 16;
   L.nhot = o;
   MJB_DATA_COLD_FIELDS(X, S)
+  MJB_DATA_CCD_FIELDS(X, S)
   L.ndbl = o;
   o = 0;
   MJB_DATA_INT_FIELDS(X, S)
@@ -275,6 +295,7 @@ struct Env {
 #undef X
 #define X(name, cnt) MJB_HD FD name() const { return FD{cd + b.L.name}; }
   MJB_DATA_COLD_FIELDS(X, _)
+  MJB_DATA_CCD_FIELDS(X, _)
 #undef X
 #define X(name, cnt) MJB_HD FI name() const { return FI{hi + b.L.name}; }
   MJB_DATA_INT_FIELDS(X, _)
