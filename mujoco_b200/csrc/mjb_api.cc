@@ -383,10 +383,10 @@ int mjb_rollout(mjbBatch* B, int nstep, unsigned int control_spec, const double*
   for (auto& s : csegs) ncontrol += s.n;
   // defaults for unspecified user inputs, initial state, warmstart, warning counters
   {
-    if (!(control_spec & ST_CTRL) || !control) field_zero(B, false, B->b.L.ctrl, B->hm.dm.sz.nu);
-    if (!(control_spec & ST_QFRC_APPLIED) || !control) field_zero(B, false, B->b.L.qfrc_applied, nv);
+    if (!(control_spec & ST_CTRL) || !control) { if (int rc = field_zero(B, false, B->b.L.ctrl, B->hm.dm.sz.nu)) return rc; }
+    if (!(control_spec & ST_QFRC_APPLIED) || !control) { if (int rc = field_zero(B, false, B->b.L.qfrc_applied, nv)) return rc; }
     if ((control_spec & ST_XFRC_APPLIED) && control) B->b.xfrc = 1;
-    else if (B->b.xfrc) field_zero(B, false, B->b.L.xfrc_applied, 6 * B->hm.dm.sz.nbody);
+    else if (B->b.xfrc) { if (int rc = field_zero(B, false, B->b.L.xfrc_applied, 6 * B->hm.dm.sz.nbody)) return rc; }
     if (B->hm.dm.sz.neq && (!(control_spec & ST_EQ_ACTIVE) || !control)) {   // rollout.cc:110-114
       const int neq = B->hm.dm.sz.neq;
       std::vector<double> ea((size_t)nenv * neq);
@@ -407,12 +407,12 @@ int mjb_rollout(mjbBatch* B, int nstep, unsigned int control_spec, const double*
       if (!(control_spec & ST_MOCAP_POS) || !control) field_from_host(B, false, B->b.L.mocap_pos, 3 * S.nmocap, mp.data());
       if (!(control_spec & ST_MOCAP_QUAT) || !control) field_from_host(B, false, B->b.L.mocap_quat, 4 * S.nmocap, mq.data());
     }
-    field_zero(B, true, B->b.L.warning, NWARNING);
+    if (int rc = field_zero(B, true, B->b.L.warning, NWARNING)) return rc;
     if (int rc = mjb_set_state(B, state0, full)) return rc;
     if (warmstart0) {
       if (int rc = mjb_set_state(B, warmstart0, ST_WARMSTART)) return rc;
     } else {
-      field_zero(B, false, B->b.L.qacc_warmstart, nv);
+      if (int rc = field_zero(B, false, B->b.L.qacc_warmstart, nv)) return rc;
     }
   }
   double* d_control = nullptr;

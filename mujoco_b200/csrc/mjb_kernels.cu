@@ -189,8 +189,10 @@ long launches() { return g_launches; }
 
 static inline int nblocks(const Batch& b, int threads) { return (b.nenv + threads - 1) / threads; }
 
+// (an empty field, e.g. ctrl of a model without actuators, launches nothing: a grid of 0 blocks is a launch error)
 int launch_pack(const Batch& b, int is_int, long off, long cnt, void* dense, int to_dense, void* s) {
   const long n = (long)b.nenv * cnt;
+  if (n == 0) return 0;
   k_pack<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)s>>>(b, is_int, off, cnt, dense, to_dense);
   g_launches++;
   CK(cudaPeekAtLastError(), "k_pack launch");
@@ -198,6 +200,7 @@ int launch_pack(const Batch& b, int is_int, long off, long cnt, void* dense, int
 }
 int launch_fill_zero(const Batch& b, int is_int, long off, long cnt, void* s) {
   const long n = (long)b.nenv * cnt;
+  if (n == 0) return 0;
   k_fill_zero<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)s>>>(b, is_int, off, cnt);
   g_launches++;
   CK(cudaPeekAtLastError(), "k_fill_zero launch");
