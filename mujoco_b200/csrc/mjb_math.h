@@ -23,7 +23,6 @@ namespace mjb {
 constexpr double kMinVal = 1e-15;   // mjMINVAL  (reference include/mujoco/mjtype.h:27)
 constexpr double kMaxVal = 1e10;    // mjMAXVAL
 constexpr double kPi = 3.14159265358979323846;
-constexpr int kMaxDenseNv = 60;     // dense-Jacobian models have nv < 60 (mj_isSparse)
 constexpr double kMinMu = 1e-5;     // mjMINMU   (include/mujoco/mjmodel.h:25-32)
 constexpr double kMinImp = 0.0001;  // mjMINIMP
 constexpr double kMaxImp = 0.9999;  // mjMAXIMP

@@ -418,6 +418,8 @@ int check_model(const mjModel* m) {
     int tt = m->actuator_trntype[i];
     if (tt != mjTRN_JOINT && tt != mjTRN_JOINTINPARENT && tt != mjTRN_TENDON && tt != mjTRN_SITE && tt != mjTRN_SLIDERCRANK) FAIL("actuator %d: body (adhesion) transmission", i);
     if ((tt == mjTRN_SITE || tt == mjTRN_SLIDERCRANK) && (m->actuator_damping[i] != 0 || m->actuator_armature[i] != 0)) FAIL("actuator %d: actuator damping / armature on a site / slider-crank transmission", i);
+    // fwd_velocity gathers the nonzero moments of such an actuator into a list of 64 (mjb_forward.h)
+    if ((tt == mjTRN_SITE || tt == mjTRN_SLIDERCRANK) && m->nv > 64) FAIL("actuator %d: site / slider-crank transmission on a model with nv > 64", i);
     if (tt != mjTRN_TENDON && tt != mjTRN_SITE && tt != mjTRN_SLIDERCRANK) {
       int jt = m->jnt_type[m->actuator_trnid[2 * i]];
       if ((jt == mjJNT_BALL || jt == mjJNT_FREE) && (m->actuator_damping[i] != 0 || m->actuator_armature[i] != 0))

@@ -9,7 +9,7 @@
 // mju_cholUpdate :104-147; mju_sqrMatTD_impl (engine_util_blas.c), mju_addToSymSparse and
 // mju_mulSymVecSparse (engine_util_sparse.c).
 //
-// Scope: dense Jacobian (nv < 60), pyramidal cones, no equality rows, one kinematic tree (so the
+// Scope: dense Jacobian (any nv), pyramidal cones, no equality rows, one kinematic tree (so the
 // constraint island, when islands are enabled, is the whole system and its dof / row order is the
 // global one: engine_island.c:455-650; only the cost scale differs, 1/trace(M) instead of
 // 1/(meaninertia*nv), engine_solver.c:2383-2394).
