@@ -161,6 +161,7 @@ mjbBatch* mjb_make_batch(const struct mjModel_* m, int nenv, int nconmax, int nj
   b.xfrc = 0;
   if (const char* ls = getenv("MJB_LANES")) { const int v = atoi(ls); if (v == 16 || v == 32) b.nlane = v; }
   if (H.sz.convex) b.nlane = 32;   // the convex narrow phase is built for the 32-lane mapping only
+  if (H.sz.spatial) b.nlane = 32;  // so are spatial tendons
   b.dpitch = ((size_t)b.L.ndbl + 15) / 16 * 16;   // env-major blocks, 128-byte aligned
   b.ipitch = ((size_t)b.L.nint + 31) / 32 * 32;
   size_t nd = b.dpitch * b.stride;
@@ -555,9 +556,11 @@ static bool find_field(const mjbBatch* B, const char* name, long* off, long* cnt
 #define X(fname, count) if (!strcmp(name, #fname)) { *off = L.fname; *cnt = (long)(count); *is_int = false; return true; }
   MJB_DATA_DBL_FIELDS(X, S)
   MJB_DATA_COLD_FIELDS(X, S)
+  MJB_DATA_WRAP_FIELDS(X, S)
 #undef X
 #define X(fname, count) if (!strcmp(name, #fname)) { *off = L.fname; *cnt = (long)(count); *is_int = true; return true; }
   MJB_DATA_INT_FIELDS(X, S)
+  MJB_DATA_WRAP_INT_FIELDS(X, S)
 #undef X
   return false;
 }
@@ -665,6 +668,15 @@ static int bridge_mjdata(mjbBatch* B, mjData* const* d, int nd, BridgeOp op) {
     for (int e = 0; e < nenv; e++) memcpy(d[e]->name, tmp.data() + (size_t)e * (cnt), sizeof(double) * (cnt)); \
   }
   MJB_MJDATA_OUT(X)
+  MJB_DATA_WRAP_FIELDS(X, S)   // spatial tendon paths (allocated only for models with spatial tendons)
+#undef X
+#define X(name, cnt)                                                                             \
+  if ((cnt) > 0) {                                                                               \
+    std::vector<int> it((size_t)nenv * (cnt));                                                   \
+    if (int rc2 = field_to_host(B, true, B->b.L.name, (cnt), it.data())) return rc2;              \
+    for (int e = 0; e < nenv; e++) memcpy(d[e]->name, it.data() + (size_t)e * (cnt), sizeof(int) * (cnt)); \
+  }
+  MJB_DATA_WRAP_INT_FIELDS(X, S)
 #undef X
   // Arena members (contact, efc_*) are NOT materialised in the reference's mjData: the arena allocator is private
   // to the reference library.  The counts are therefore published as zero - an mjData that claims ncon contacts

@@ -296,6 +296,69 @@ MJB_HD void gravcomp(const Env& d) {
   MJB_PSYNC();
 }
 
+#if defined(MJB_SPATIAL_UNIT) || !defined(__CUDA_ARCH__)
+// d/dt(ten_J) . vec for a spatial tendon without geom wrapping (mj_tendonDot, engine_core_smooth.c:1115-1250, dense
+// branch): per segment between different bodies, the Jacobian-derivative difference along the unit direction plus the
+// Jacobian difference along the direction's rate of change, each dotted with vec and divided by the pulley divisor
+MJB_HD double tendon_dot(const Env& d, int i, FD vec) {
+  const DModel& m = d.m;
+  const int nv = m.sz.nv, adr = m.tendon_adr[i], num = m.tendon_num[i];
+  if (m.wrap_type[adr] == WRAP_JOINT) return 0;
+  FD sx = d.site_xpos();
+  double res = 0, divisor = 1;
+  for (int j = 0; j < num - 1; j++) {
+    const int t0 = m.wrap_type[adr + j], t1 = m.wrap_type[adr + j + 1];
+    if (t0 == WRAP_PULLEY || t1 == WRAP_PULLEY) {
+      if (t0 == WRAP_PULLEY) divisor = m.wrap_prm[adr + j];
+      continue;
+    }
+    const int id0 = m.wrap_objid[adr + j], id1 = m.wrap_objid[adr + j + 1];
+    const int b0 = m.site_bodyid[id0], b1 = m.site_bodyid[id1];
+    if (b0 == b1) continue;
+    const V3 p0 = ld3(sx, 3 * id0), p1 = ld3(sx, 3 * id1);
+    V3 ang, v0, v1;
+    object_velocity(d, SOBJ_SITE, id0, ang, v0);
+    object_velocity(d, SOBJ_SITE, id1, ang, v1);
+    V3 dp = p1 - p0;
+    const double norm = normalize(dp);
+    V3 dv = v1 - v0;
+    dv = addscl(dv, dp, -dot(dp, dv));
+    dv = dv * (norm > kMinVal ? 1 / norm : 0);
+    // chain rule, first term: d/dt(jac2 - jac1) * dpnt; second term: (jac2 - jac1) * d/dt(dpnt) (mju_mulMatTVec)
+    res += dot_ref(nv, [&](int c) {
+      double t = 0;
+      for (int r = 0; r < 3; r++) { const double s = get(dp, r); if (s) t += (jacdot_elem(d, p1, b1, r, c) - jacdot_elem(d, p0, b0, r, c)) * s; }
+      return t;
+    }, [&](int c) { return vec[c]; }) / divisor;
+    res += dot_ref(nv, [&](int c) {
+      double t = 0;
+      for (int r = 0; r < 3; r++) { const double s = get(dv, r); if (s) t += (jac_elem(d, p1, b1, r, c) - jac_elem(d, p0, b0, r, c)) * s; }
+      return t;
+    }, [&](int c) { return vec[c]; }) / divisor;
+  }
+  return res;
+}
+
+// tendon-armature bias (mj_tendonBias, engine_core_smooth.c:2606-2640): qfrc_bias += ten_J * armature *
+// (d/dt(ten_J) . qvel), armature = tendon armature + the armature of actuators on the tendon; tendons in order
+MJB_HD void tendon_bias(const Env& d) {
+  const DModel& m = d.m;
+  MJB_LANE0 {
+    FD qfrc = d.qfrc_bias(), tJ = d.ten_J();
+    for (int i = 0; i < m.sz.ntendon; i++) {
+      const double armature = m.tendon_armature_eff[i];
+      if (!armature) continue;
+      const double coef = armature * tendon_dot(d, i, d.qvel());
+      if (coef) {
+        const int adr = m.ten_J_rowadr[i], nnz = m.ten_J_rownnz[i];
+        for (int j = 0; j < nnz; j++) qfrc[m.ten_J_colind[adr + j]] += coef * tJ[adr + j];
+      }
+    }
+  }
+  MJB_PSYNC();
+}
+#endif
+
 MJB_HD void fwd_velocity(const Env& d) {
   const DModel& m = d.m;
   FD qvel = d.qvel();
@@ -335,7 +398,10 @@ MJB_HD void fwd_velocity(const Env& d) {
   gravcomp(d);
   reference_constraint(d);
   rne_bias(d);
-  // tendon-armature bias: needs d/dt(ten_J), identically zero for fixed tendons -> no contribution
+  // tendon-armature bias: d/dt(ten_J) is identically zero for fixed tendons, so only spatial tendons contribute
+#if defined(MJB_SPATIAL_UNIT) || !defined(__CUDA_ARCH__)
+  if (d.feat & FEAT_SPATIAL) tendon_bias(d);
+#endif
 }
 
 // muscle model (engine_util_misc.c:1049-1190): FLV gain, passive bias, activation dynamics

@@ -208,9 +208,10 @@ int launch_fill_zero(const Batch& b, int is_int, long off, long cnt, void* s) {
 }
 
 // lean kernels (FEAT = 0) when the model needs none of the optional pipeline parts (FEAT_*); a model with convex
-// collision pairs is never lean, since only the FEAT_CONVEX instantiations carry its narrow phase
+// collision pairs or spatial tendons is never lean, since only the FEAT_CONVEX / FEAT_SPATIAL instantiations carry
+// their code
 static bool lean_model(const DModel& dm, const Batch& b) {
-  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc && !dm.sz.convex;
+  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc && !dm.sz.convex && !dm.sz.spatial;
 }
 
 // split step: position + velocity | PGS (4 lanes per environment, mjb_pgs4.cu) | finish + integrate | redo
@@ -219,7 +220,7 @@ bool split_step_available(const DModel& dm, const Batch& b) {
   static int want = -1;
   if (want < 0) { const char* s = getenv("MJB_SPLIT"); want = s ? atoi(s) : 1; }
   const bool islands = dm.sz.ntree > 1 && !(dm.opt.disableflags & DSBL_ISLAND);
-  return want && b.warp_per_env && b.nlane == 32 && !dm.sz.convex && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
+  return want && b.warp_per_env && b.nlane == 32 && !dm.sz.convex && !dm.sz.spatial && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
          (dm.opt.integrator == INT_EULER || dm.opt.integrator == INT_IMPLICITFAST);
 }
 int launch_split_step(const DModel& dm, const Batch& b, int first, int later, void* s, void* stagger) {
@@ -299,7 +300,9 @@ int profile_split_step(const DModel& dm, const Batch& b, void* s, float* ms) {
 }
 
 int launch_stages(const DModel& dm, const Batch& b, int mask, int flags, void* s) {
-  if (dm.sz.convex) {   // convex collision pairs: only these instantiations carry GJK / EPA (32 lanes or one lane per env)
+  if (dm.sz.spatial) {   // spatial tendons: only these instantiations carry the tendon paths (32 lanes or one lane per env)
+    if (b.warp_per_env) launch_kstep_spatial32(dm, b, mask, flags, s); else launch_kstep_lane_spatial(dm, b, mask, flags, s);
+  } else if (dm.sz.convex) {   // convex collision pairs: only these instantiations carry GJK / EPA (32 lanes or one lane per env)
     if (b.warp_per_env) launch_kstep_convex32(dm, b, mask, flags, s); else launch_kstep_lane_convex(dm, b, mask, flags, s);
   } else if (b.warp_per_env) {
     // lean kernels when the model needs none of the optional pipeline parts (FEAT_*)

@@ -18,6 +18,10 @@ void launch_kstep_any16(const DModel& dm, const Batch& b, int mask, int flags, v
 // validation mapping (mjb_kstep_convex32.cu)
 void launch_kstep_convex32(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
 void launch_kstep_lane_convex(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
+// spatial tendons (FEAT_ALL | FEAT_SPATIAL, solver chosen at run time): fused 32-lane kernel and the lane-per-env
+// validation mapping (mjb_kstep_spatial32.cu)
+void launch_kstep_spatial32(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
+void launch_kstep_lane_spatial(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
 // lean instantiations (FEAT = 0): models without sensors, equalities, several trees or implicitfast
 void launch_kstep_pgs32_lean(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
 void launch_kstep_newton32_lean(const DModel& dm, const Batch& b, int mask, int flags, void* stream);

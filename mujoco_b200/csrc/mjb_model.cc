@@ -410,9 +410,6 @@ int check_model(const mjModel* m) {
   for (int i = 0; i < m->ngeom; i++) {
     if (m->geom_adhesion[i] != 0) FAIL("geom adhesion");
   }
-  for (int i = 0; i < m->ntendon; i++) {
-    if (m->wrap_type[m->tendon_adr[i]] != mjWRAP_JOINT) FAIL("spatial tendons");
-  }
   if (m->nout != m->nu || m->nactuator != m->nu) FAIL("multi-input/multi-output actuators");
   for (int i = 0; i < m->nactuator; i++) {
     int tt = m->actuator_trntype[i];
@@ -618,6 +615,22 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
   B.addI(&D.ten_J_rownnz, m->ten_J_rownnz, m->ntendon);
   B.addI(&D.ten_J_rowadr, m->ten_J_rowadr, m->ntendon);
   B.addI(&D.ten_J_colind, m->ten_J_colind, m->nJten);
+  {   // spatial tendons (mj_tendon, engine_core_smooth.c:985-1109): each tendon's path points are first written to a
+      // slot of its own in wrap_xpos / wrap_obj, then packed to the running count ten_wrapadr.  A site or a pulley
+      // gives at most one point and a wrapping geom at most two, so the slots fit the 2*nwrap points of mjData.
+    S.spatial = 0;
+    std::vector<int> slot(m->ntendon);
+    int adr = 0;
+    for (int i = 0; i < m->ntendon; i++) {
+      slot[i] = adr;
+      const int a = m->tendon_adr[i], n = m->tendon_num[i];
+      if (m->wrap_type[a] == mjWRAP_JOINT) continue;
+      S.spatial = 1;
+      for (int j = 0; j < n; j++) adr += (m->wrap_type[a + j] == mjWRAP_SPHERE || m->wrap_type[a + j] == mjWRAP_CYLINDER) ? 2 : 1;
+    }
+    B.addI(&D.tendon_slotadr, slot.data(), m->ntendon);
+    B.addI(&D.body_simple, m->body_simple, m->nbody);
+  }
   {
     std::vector<int> trn(m->nu);
     for (int i = 0; i < m->nu; i++) trn[i] = m->actuator_trnid[2 * i];
@@ -740,6 +753,13 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
       tdmp[i] = m->tendon_damping[i] + act_damping(m, true, i, poly);
       for (int k = 0; k < mjNPOLY; k++) tpoly[mjNPOLY * i + k] = poly[k];
       tarm[i] = m->tendon_armature[i] + act_armature(m, true, i);
+      // mj_tendonDot (the bias of tendon armature) has no geom-wrapping branch in the reference either
+      if (tarm[i] != 0 && m->wrap_type[m->tendon_adr[i]] != mjWRAP_JOINT)
+        for (int j = 0; j < m->tendon_num[i]; j++)
+          if (m->wrap_type[m->tendon_adr[i] + j] == mjWRAP_SPHERE || m->wrap_type[m->tendon_adr[i] + j] == mjWRAP_CYLINDER) {
+            set_error("unsupported: tendon armature (incl. actuator armature) on a spatial tendon with geom wrapping");
+            return -2;
+          }
     }
     B.addD(&D.tendon_damping_eff, tdmp.data(), m->ntendon);
     B.addD(&D.tendon_dampingpoly_eff, tpoly.data(), mjNPOLY * m->ntendon);
@@ -957,6 +977,10 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
     }
   }
   S.npair = (int)pg1.size();
+  if (S.spatial && S.convex) {
+    set_error("unsupported: spatial tendons together with convex (GJK / EPA) collision pairs: no kernel carries both");
+    return -2;
+  }
   // polytope scratch of the GJK candidates (mjb_convex.h): kCcdSlots slots per environment, fewer when the model has
   // fewer GJK candidates; nothing at all for models without them, whose layout is unchanged
   S.ccdslots = std::min(kCcdSlots, S.nconvex);

@@ -207,8 +207,362 @@ MJB_HD void com_pos(const Env& d) {
   MJB_PSYNC();
 }
 
+#if defined(MJB_SPATIAL_UNIT) || !defined(__CUDA_ARCH__)
 // ------------------------------------------------------------------------------------------------
-// fixed tendons: length and constant-pattern sparse Jacobian
+// spatial tendons (FEAT_SPATIAL): compiled on the device only in mjb_kstep_spatial32.cu, so that every other kernel
+// keeps its code.  Wrapping: mju_wrap, wrap_circle, wrap_inside, is_intersect, length_circle
+// (engine_util_misc.c:35-417); 2D vectors are double[2], dot products in mju_dot's order.
+MJB_HD double dot2(const double* a, const double* b) {
+  return dot_ref(2, [&](int i) { return a[i]; }, [&](int i) { return b[i]; });
+}
+MJB_HD double normalize2(double* v) {   // mju_normalize, n = 2
+  const double n = sqrt(dot2(v, v));
+  if (n < kMinVal) { v[0] = 1; v[1] = 0; }
+  else { const double inv = 1 / n; v[0] *= inv; v[1] *= inv; }
+  return n;
+}
+MJB_HD bool wrap_is_intersect(const double* p1, const double* p2, const double* p3, const double* p4) {
+  const double det = (p4[1] - p3[1]) * (p2[0] - p1[0]) - (p4[0] - p3[0]) * (p2[1] - p1[1]);
+  if (fabs(det) < kMinVal) return false;
+  const double a = ((p4[0] - p3[0]) * (p1[1] - p3[1]) - (p4[1] - p3[1]) * (p1[0] - p3[0])) / det;
+  const double b = ((p2[0] - p1[0]) * (p1[1] - p3[1]) - (p2[1] - p1[1]) * (p1[0] - p3[0])) / det;
+  return a >= 0 && a <= 1 && b >= 0 && b <= 1;
+}
+MJB_HD double wrap_length_circle(const double* p0, const double* p1, int ind, double radius) {
+  double p0n[2] = {p0[0], p0[1]}, p1n[2] = {p1[0], p1[1]};
+  normalize2(p0n);
+  normalize2(p1n);
+  double angle = acos(dot2(p0n, p1n));
+  const double cr = p0[1] * p1[0] - p0[0] * p1[1];
+  if ((cr > 0 && ind) || (cr < 0 && !ind)) angle = 2 * kPi - angle;
+  return radius * angle;
+}
+// circle wrap of the 2D segment end[0..1] - end[2..3]; side: optional 2D side point.  Length or -1 (no wrap)
+MJB_HD double wrap_circle(double* pnt, const double* end, const double* side, double radius) {
+  const double sqlen0 = end[0] * end[0] + end[1] * end[1];
+  const double sqlen1 = end[2] * end[2] + end[3] * end[3];
+  const double sqrad = radius * radius;
+  if (sqlen0 < sqrad || sqlen1 < sqrad || radius < kMinVal) return -1;
+  const double dif[2] = {end[2] - end[0], end[3] - end[1]};
+  const double dd = dif[0] * dif[0] + dif[1] * dif[1];
+  if (dd < kMinVal) return -1;
+  double a = -(dif[0] * end[0] + dif[1] * end[1]) / dd;
+  if (a < 0) a = 0;
+  else if (a > 1) a = 1;
+  double tmp[2] = {a * dif[0] + end[0], a * dif[1] + end[1]};
+  if (tmp[0] * tmp[0] + tmp[1] * tmp[1] > sqrad && (!side || dot2(side, tmp) >= 0)) return -1;
+  const double sqrt0 = sqrt(sqlen0 - sqrad), sqrt1 = sqrt(sqlen1 - sqrad);
+  double sol[2][2][2], good[2];
+  for (int i = 0; i < 2; i++) {
+    const double sgn = (i == 0 ? 1 : -1);
+    sol[i][0][0] = (end[0] * sqrad + sgn * radius * end[1] * sqrt0) / sqlen0;
+    sol[i][0][1] = (end[1] * sqrad - sgn * radius * end[0] * sqrt0) / sqlen0;
+    sol[i][1][0] = (end[2] * sqrad - sgn * radius * end[3] * sqrt1) / sqlen1;
+    sol[i][1][1] = (end[3] * sqrad + sgn * radius * end[2] * sqrt1) / sqlen1;
+    if (side) {
+      tmp[0] = sol[i][0][0] + sol[i][1][0]; tmp[1] = sol[i][0][1] + sol[i][1][1];
+      normalize2(tmp);
+      good[i] = dot2(tmp, side);
+    } else {
+      tmp[0] = sol[i][0][0] - sol[i][1][0]; tmp[1] = sol[i][0][1] - sol[i][1][1];
+      good[i] = -dot2(tmp, tmp);
+    }
+    if (wrap_is_intersect(end, sol[i][0], end + 2, sol[i][1])) good[i] = -10000;
+  }
+  const int i = (good[0] > good[1] ? 0 : 1);
+  pnt[0] = sol[i][0][0]; pnt[1] = sol[i][0][1]; pnt[2] = sol[i][1][0]; pnt[3] = sol[i][1][1];
+  if (wrap_is_intersect(end, pnt, end + 2, pnt + 2)) return -1;
+  return wrap_length_circle(sol[i][0], sol[i][1], i, radius);
+}
+// wrap with the side site inside the circle: Newton iteration on asin(A z) + asin(B z) - 2 asin(z) + G = 0.
+// 0 (both points at the same tangent point) or -1 (no wrap)
+MJB_HD double wrap_inside(double* pnt, const double* end, double radius) {
+  const int maxiter = 20;
+  const double zinit = 1 - 1e-7, tolerance = 1e-6;
+  const double len0 = sqrt(dot2(end, end)), len1 = sqrt(dot2(end + 2, end + 2));
+  const double dif[2] = {end[2] - end[0], end[3] - end[1]};
+  const double dd = dif[0] * dif[0] + dif[1] * dif[1];
+  if (len0 <= radius || len1 <= radius || radius < kMinVal || len0 < kMinVal || len1 < kMinVal) return -1;
+  if (dd > kMinVal) {
+    const double a = -(dif[0] * end[0] + dif[1] * end[1]) / dd;
+    if (a > 0 && a < 1) {
+      const double tmp[2] = {end[0] + dif[0] * a, end[1] + dif[1] * a};
+      if (sqrt(dot2(tmp, tmp)) <= radius) return -1;
+    }
+  }
+  pnt[0] = 0.5 * (end[0] + end[2]);
+  pnt[1] = 0.5 * (end[1] + end[3]);
+  normalize2(pnt);
+  pnt[0] = pnt[0] * radius; pnt[1] = pnt[1] * radius;
+  pnt[2] = pnt[0]; pnt[3] = pnt[1];
+  const double A = radius / len0, B = radius / len1;
+  const double cosG = (len0 * len0 + len1 * len1 - dd) / (2 * len0 * len1);
+  if (cosG < -1 + kMinVal) return -1;
+  else if (cosG > 1 - kMinVal) return 0;
+  const double G = acos(cosG);
+  double z = zinit;
+  double f = asin(A * z) + asin(B * z) - 2 * asin(z) + G;
+  if (f > 0) return 0;
+  int iter;
+  for (iter = 0; iter < maxiter && fabs(f) > tolerance; iter++) {
+    const double df = A / dmax(kMinVal, sqrt(1 - z * z * A * A)) + B / dmax(kMinVal, sqrt(1 - z * z * B * B)) -
+                      2 / dmax(kMinVal, sqrt(1 - z * z));
+    if (df > -kMinVal) return 0;
+    const double z1 = z - f / df;
+    if (z1 > z) return 0;
+    z = z1;
+    f = asin(A * z) + asin(B * z) - 2 * asin(z) + G;
+    if (f > tolerance) return 0;
+  }
+  if (iter >= maxiter) return 0;
+  double vec[2], ang;
+  if (end[0] * end[3] - end[1] * end[2] > 0) { vec[0] = end[0]; vec[1] = end[1]; ang = asin(z) - asin(A * z); }
+  else { vec[0] = end[2]; vec[1] = end[3]; ang = asin(z) - asin(B * z); }
+  normalize2(vec);
+  pnt[0] = radius * (cos(ang) * vec[0] - sin(ang) * vec[1]);
+  pnt[1] = radius * (sin(ang) * vec[0] + cos(ang) * vec[1]);
+  pnt[2] = pnt[0]; pnt[3] = pnt[1];
+  return 0;
+}
+MJB_HD V3 mul_mat_t(const M3& a, V3 v) {   // mju_mulMatTVec3
+  return V3{a.m[0] * v.x + a.m[3] * v.y + a.m[6] * v.z, a.m[1] * v.x + a.m[4] * v.y + a.m[7] * v.z,
+            a.m[2] * v.x + a.m[5] * v.y + a.m[8] * v.z};
+}
+// mju_wrap: the path x0 -> x1 around a sphere / cylinder (geom frame xpos, xmat), optional side site.  Returns the
+// wrap length and the two tangent points w0, w1, or -1 when the straight segment does not touch the geom
+MJB_HD double wrap_geom(V3& w0, V3& w1, V3 x0, V3 x1, V3 xpos, const M3& xmat, double radius, int type,
+                        const V3* side) {
+  const V3 p0 = mul_mat_t(xmat, x0 - xpos), p1 = mul_mat_t(xmat, x1 - xpos);
+  if (sqrt(dot(p0, p0)) < kMinVal || sqrt(dot(p1, p1)) < kMinVal) return -1;
+  V3 ax0, ax1;
+  if (type == WRAP_SPHERE) {
+    ax0 = p0;
+    normalize(ax0);
+    V3 normal = cross(p0, p1);
+    const double nrm = normalize(normal);
+    if (nrm < kMinVal) {   // p0, p1 parallel
+      int i = 0;
+      if (fabs(ax0.y) > fabs(ax0.x) && fabs(ax0.y) > fabs(ax0.z)) i = 1;
+      if (fabs(ax0.z) > fabs(ax0.x) && fabs(ax0.z) > fabs(ax0.y)) i = 2;
+      ax1 = V3{i == 0 ? 0.0 : 1.0, i == 1 ? 0.0 : 1.0, i == 2 ? 0.0 : 1.0};
+      normal = cross(ax0, ax1);
+      normalize(normal);
+    }
+    ax1 = cross(normal, ax0);
+    normalize(ax1);
+  } else {
+    ax0 = V3{1, 0, 0};
+    ax1 = V3{0, 1, 0};
+  }
+  const double dd[4] = {dot(p0, ax0), dot(p0, ax1), dot(p1, ax0), dot(p1, ax1)};
+  V3 s{0, 0, 0};
+  double sd[2] = {0, 0};
+  if (side) {
+    s = mul_mat_t(xmat, *side - xpos);
+    sd[0] = dot(s, ax0); sd[1] = dot(s, ax1);
+    normalize2(sd);
+    sd[0] = sd[0] * radius; sd[1] = sd[1] * radius;
+  }
+  double wlen, pnt[4];
+  if (side && sqrt(dot(s, s)) < radius) wlen = wrap_inside(pnt, dd, radius);
+  else wlen = wrap_circle(pnt, dd, side ? sd : nullptr, radius);
+  if (wlen < 0) return -1;
+  V3 r0 = ax0 * pnt[0], r1 = ax0 * pnt[2];
+  r0 = r0 + ax1 * pnt[1];
+  r1 = r1 + ax1 * pnt[3];
+  if (type == WRAP_CYLINDER) {
+    const double L0 = sqrt((p0.x - r0.x) * (p0.x - r0.x) + (p0.y - r0.y) * (p0.y - r0.y));
+    const double L1 = sqrt((p1.x - r1.x) * (p1.x - r1.x) + (p1.y - r1.y) * (p1.y - r1.y));
+    r0.z = p0.z + (p1.z - p0.z) * L0 / (L0 + wlen + L1);
+    r1.z = p0.z + (p1.z - p0.z) * (L0 + wlen) / (L0 + wlen + L1);
+    const double height = fabs(r1.z - r0.z);
+    wlen = sqrt(wlen * wlen + height * height);
+  }
+  w0 = mulmv(xmat, r0) + xpos;
+  w1 = mulmv(xmat, r1) + xpos;
+  return wlen;
+}
+MJB_HD double jac_elem(const Env& d, V3 pt, int body, int k, int c);   // mjb_constraint.h
+MJB_HD double dist3(V3 a, V3 b) { const V3 d = a - b; return sqrt(d.x * d.x + d.y * d.y + d.z * d.z); }
+
+// phase 1, one lane per spatial tendon: walk the path (mj_tendon, engine_core_smooth.c:985-1109) for the length and
+// the path points.  The points go to the tendon's own slot (tendon_slotadr) in wrap_xpos / wrap_obj, since the running
+// count ten_wrapadr depends on which wraps of the earlier tendons are active; ten_wrapnum holds the count.
+MJB_HD void tendon_path(const Env& d, int i) {
+  const DModel& m = d.m;
+  FD sx = d.site_xpos(), gx = d.geom_xpos(), gm = d.geom_xmat(), wx = d.wrap_xpos();
+  FI wo = d.wrap_obj();
+  const int adr = m.tendon_adr[i], num = m.tendon_num[i], w0 = m.tendon_slotadr[i];
+  int w = w0, j = 0;
+  double len = 0, divisor = 1;
+  while (j < num - 1) {
+    int t1 = m.wrap_type[adr + j + 1], id1 = m.wrap_objid[adr + j + 1];
+    const int t0 = m.wrap_type[adr + j], id0 = m.wrap_objid[adr + j];
+    if (t0 == WRAP_PULLEY || t1 == WRAP_PULLEY) {
+      if (t0 == WRAP_PULLEY) {
+        divisor = m.wrap_prm[adr + j];
+        st3(wx, 3 * w, V3{0, 0, 0});
+        wo[w++] = -2;
+      }
+      j++;
+      continue;
+    }
+    const V3 p0 = ld3(sx, 3 * id0);
+    double wlen = -1;
+    int wrapid = -1;
+    const bool geom = (t1 == WRAP_SPHERE || t1 == WRAP_CYLINDER);
+    V3 a, b;
+    if (geom) {
+      wrapid = id1;
+      id1 = m.wrap_objid[adr + j + 2];
+      const int sideid = round_int(m.wrap_prm[adr + j + 1]);
+      const V3 side = sideid >= 0 ? ld3(sx, 3 * sideid) : V3{0, 0, 0};
+      wlen = wrap_geom(a, b, p0, ld3(sx, 3 * id1), ld3(gx, 3 * wrapid), ld9(gm, 9 * wrapid), m.geom_size[3 * wrapid], t1,
+                       sideid >= 0 ? &side : nullptr);
+    }
+    const V3 p1 = ld3(sx, 3 * id1);
+    if (wlen < 0) len += dist3(p0, p1) / divisor;
+    else len += (dist3(p0, a) + wlen + dist3(b, p1)) / divisor;
+    st3(wx, 3 * w, p0);
+    wo[w] = -1;
+    if (wlen >= 0) {
+      st3(wx, 3 * (w + 1), a);
+      st3(wx, 3 * (w + 2), b);
+      wo[w + 1] = wrapid; wo[w + 2] = wrapid;
+    }
+    w += (wlen < 0 ? 1 : 3);
+    j += (geom ? 2 : 1);
+    if (j == num - 1 || m.wrap_type[adr + j + 1] == WRAP_PULLEY) {   // last site before a pulley or the end
+      st3(wx, 3 * w, p1);
+      wo[w++] = -1;
+    }
+  }
+  d.ten_length()[i] = len;
+  d.ten_wrapnum()[i] = w - w0;
+}
+
+// tendon Jacobian entry (tendon i, row element a, column c) from one path segment q1 (body b1) -> q2 (body b2): the
+// chain rule of mj_tendon with mj_jacDifPair (engine_core_util.c:437-516, issparse = 1), mju_mulMatTVec and
+// mju_combineSparseInc (engine_util_sparse.c:309), for this one element.  J is the element so far; scl = 1/divisor.
+MJB_HD double segment_entry(const Env& d, int i, int a, int c, double J, V3 q1, int b1, V3 q2, int b2, double scl) {
+  const DModel& m = d.m;
+  const int nv = m.sz.nv;
+  V3 dif = q2 - q1;
+  normalize(dif);
+  const bool simple = m.body_simple[b1] && m.body_simple[b2];
+  // the merged dof chain (mj_mergeChainSimple / mj_mergeChain), increasing: NV and membership
+  auto in_chain = [&](int k) -> bool {
+    if (simple) return (k >= m.body_dofadr[b1] && k < m.body_dofadr[b1] + m.body_dofnum[b1]) ||
+                       (k >= m.body_dofadr[b2] && k < m.body_dofadr[b2] + m.body_dofnum[b2]);
+    return m.body_dofanc[(long)b1 * nv + k] || m.body_dofanc[(long)b2 * nv + k];
+  };
+  int NV = 0;
+  if (simple) NV = m.body_dofnum[b1] + m.body_dofnum[b2];
+  else for (int k = 0; k < nv; k++) NV += in_chain(k);
+  if (!NV) return J;
+  // column k of (jac2 - jac1) . dif, zero components of dif skipped.  Simple bodies write -(first) and +(second)
+  // straight into the difference (mj_jacSparseSimple); otherwise jac2 - jac1 of the two chain Jacobians.
+  auto chain_rule = [&](int k) -> double {
+    double jd[3];
+    if (simple) {
+      const bool second = k >= m.body_dofadr[b2] && k < m.body_dofadr[b2] + m.body_dofnum[b2];
+      const V3 pt = second ? q2 : q1;
+      const int body = second ? b2 : b1;
+      const V3 off = pt - ld3(d.subtree_com(), 3 * m.body_rootid[body]);
+      const V3 t = cross(ld3(d.cdof(), 6 * k), off);
+      for (int r = 0; r < 3; r++) {
+        const double v = d.cdof()[6 * k + 3 + r] + get(t, r);
+        jd[r] = second ? v : -v;
+      }
+    } else {
+      for (int r = 0; r < 3; r++) jd[r] = jac_elem(d, q2, b2, r, k) - jac_elem(d, q1, b1, r, k);
+    }
+    double res = 0;
+    for (int r = 0; r < 3; r++) { const double s = get(dif, r); if (s) res += jd[r] * s; }
+    return res;
+  };
+  const int radr = m.ten_J_rowadr[i], rnnz = m.ten_J_rownnz[i];
+  bool same = (NV == rnnz);
+  for (int e = 0; e < rnnz && same; e++) same = in_chain(m.ten_J_colind[radr + e]);
+  if (same) {   // identical pattern: dst = 1*dst + scl*src, element for element (mju_addToSclScl)
+    int k = 0, n = -1;   // the a-th dof of the chain
+    for (; k < nv; k++) if (in_chain(k) && ++n == a) break;
+    return J * 1.0 + chain_rule(k) * scl;
+  }
+  if (!in_chain(c)) return J;   // merge: only common indices change
+  return J + scl * chain_rule(c);
+}
+
+// phase 2, one lane per element of a spatial tendon's ten_J row: the element's segments in path order, with the
+// points of phase 1 (sites from site_xpos, tangent points from the tendon's slot)
+MJB_HD void tendon_jacobian(const Env& d) {
+  const DModel& m = d.m;
+  FD J = d.ten_J(), sx = d.site_xpos(), wx = d.wrap_xpos();
+  FI wo = d.wrap_obj();
+  MJB_PFOR(q, m.sz.nJten) {
+    int i = 0;
+    while (i + 1 < m.sz.ntendon && m.ten_J_rowadr[i + 1] <= q) i++;
+    const int adr = m.tendon_adr[i], num = m.tendon_num[i];
+    if (m.wrap_type[adr] == WRAP_JOINT) continue;
+    const int a = q - m.ten_J_rowadr[i], c = m.ten_J_colind[q];
+    double val = 0, divisor = 1;
+    int w = m.tendon_slotadr[i], j = 0;
+    while (j < num - 1) {
+      const int t0 = m.wrap_type[adr + j], t1 = m.wrap_type[adr + j + 1];
+      if (t0 == WRAP_PULLEY || t1 == WRAP_PULLEY) {
+        if (t0 == WRAP_PULLEY) { divisor = m.wrap_prm[adr + j]; w++; }
+        j++;
+        continue;
+      }
+      const bool geom = (t1 == WRAP_SPHERE || t1 == WRAP_CYLINDER);
+      const int id0 = m.wrap_objid[adr + j], id1 = m.wrap_objid[adr + j + (geom ? 2 : 1)];
+      const bool wrapped = geom && wo[w + 1] >= 0;
+      V3 pt[4];
+      int bd[4];
+      pt[0] = ld3(sx, 3 * id0); bd[0] = m.site_bodyid[id0];
+      const int np = wrapped ? 4 : 2;
+      if (wrapped) {
+        pt[1] = ld3(wx, 3 * (w + 1)); pt[2] = ld3(wx, 3 * (w + 2));
+        bd[1] = bd[2] = m.geom_bodyid[m.wrap_objid[adr + j + 1]];
+      }
+      pt[np - 1] = ld3(sx, 3 * id1); bd[np - 1] = m.site_bodyid[id1];
+      for (int k = 0; k + 1 < np; k++)
+        if (bd[k] != bd[k + 1]) val = segment_entry(d, i, a, c, val, pt[k], bd[k], pt[k + 1], bd[k + 1], 1 / divisor);
+      w += wrapped ? 3 : 1;
+      j += geom ? 2 : 1;
+      if (j == num - 1 || m.wrap_type[adr + j + 1] == WRAP_PULLEY) w++;
+    }
+    J[q] = val;
+  }
+}
+
+// ten_wrapadr as the running count over the tendons, and each spatial tendon's points packed from its slot to there
+// (slots never start before the packed position, so one forward pass moves them in place)
+MJB_HD void tendon_pack(const Env& d) {
+  const DModel& m = d.m;
+  MJB_LANE0 {
+    FD wx = d.wrap_xpos();
+    FI wo = d.wrap_obj(), wadr = d.ten_wrapadr(), wnum = d.ten_wrapnum();
+    int cnt = 0;
+    for (int i = 0; i < m.sz.ntendon; i++) {
+      const bool spatial = m.wrap_type[m.tendon_adr[i]] != WRAP_JOINT;
+      const int n = spatial ? wnum[i] : 0, s = m.tendon_slotadr[i];
+      wadr[i] = cnt;
+      wnum[i] = n;
+      for (int k = 0; k < n; k++) {
+        for (int r = 0; r < 3; r++) wx[3 * (cnt + k) + r] = wx[3 * (s + k) + r];
+        wo[cnt + k] = wo[s + k];
+      }
+      cnt += n;
+    }
+  }
+  MJB_PSYNC();
+}
+#endif
+
+// ------------------------------------------------------------------------------------------------
+// tendons: length and sparse Jacobian.  Fixed tendons: constant pattern, one lane per tendon.  Spatial tendons
+// (FEAT_SPATIAL): path walk per tendon, then the Jacobian elements spread over the lanes, then the path packing.
 MJB_HD void tendon(const Env& d) {
   const DModel& m = d.m;
   const int nt = m.sz.ntendon;
@@ -216,6 +570,9 @@ MJB_HD void tendon(const Env& d) {
   FD L = d.ten_length(), J = d.ten_J(), qpos = d.qpos();
   MJB_PFOR(i, nt) {
     const int adr = m.tendon_adr[i], num = m.tendon_num[i];
+#if defined(MJB_SPATIAL_UNIT) || !defined(__CUDA_ARCH__)
+    if ((d.feat & FEAT_SPATIAL) && m.wrap_type[adr] != WRAP_JOINT) { tendon_path(d, i); continue; }
+#endif
     const int radr = m.ten_J_rowadr[i], rnnz = m.ten_J_rownnz[i];
     double len = 0;
     for (int a = 0; a < rnnz; a++) J[radr + a] = 0;
@@ -232,6 +589,13 @@ MJB_HD void tendon(const Env& d) {
     L[i] = len;
   }
   MJB_PSYNC();
+#if defined(MJB_SPATIAL_UNIT) || !defined(__CUDA_ARCH__)
+  if (d.feat & FEAT_SPATIAL) {
+    tendon_jacobian(d);
+    MJB_PSYNC();
+    tendon_pack(d);
+  }
+#endif
 }
 
 // ------------------------------------------------------------------------------------------------

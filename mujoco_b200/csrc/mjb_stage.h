@@ -100,9 +100,11 @@ MJB_HD void run_env(const DModel& m, const Batch& b, int e, int mask, int flags,
   Env d(m, b, e, lane, nlane);
 #if !defined(__CUDA_ARCH__)
   // a host compilation of this code (the emulation of the device path) is one build for every model: a model with
-  // convex collision pairs takes the convex narrow phase there too.  Device kernels fix their features per
-  // instantiation instead (FEAT_CONVEX only in mjb_kstep_convex32.cu).
+  // convex collision pairs takes the convex narrow phase there too, and one with spatial tendons their paths.  Device
+  // kernels fix their features per instantiation instead (FEAT_CONVEX only in mjb_kstep_convex32.cu, FEAT_SPATIAL
+  // only in mjb_kstep_spatial32.cu).
   if (m.sz.convex) feat |= FEAT_CONVEX;
+  if (m.sz.spatial) feat |= FEAT_SPATIAL;
 #endif
   d.sm = sm; d.smcap = smcap; d.mask = lanes; d.feat = feat;
   d.solver = solver < 0 ? m.opt.solver : solver;
