@@ -82,8 +82,9 @@ MJB_API int mjb_nenv(const mjbBatch* b);
 MJB_API int mjb_reset(mjbBatch* b);
 
 /* state I/O with the reference's signature semantics; supported bits: mjSTATE_TIME, QPOS, QVEL,
- * ACT, WARMSTART, CTRL, QFRC_APPLIED, XFRC_APPLIED, MOCAP_POS, MOCAP_QUAT,  (mjSTATE_FULLPHYSICS =
- * TIME|QPOS|QVEL|ACT|...), EQ_ACTIVE (0 / 1 as doubles, like mj_setState).  Once xfrc_applied has been written the
+ * ACT, HISTORY (the nhistory doubles of the actuator and sensor history buffers, mjData.history), WARMSTART, CTRL,
+ * QFRC_APPLIED, XFRC_APPLIED, MOCAP_POS, MOCAP_QUAT,  (mjSTATE_FULLPHYSICS = TIME|QPOS|QVEL|ACT|HISTORY|...),
+ * EQ_ACTIVE (0 / 1 as doubles, like mj_setState).  Once xfrc_applied has been written the
  * batch steps with the full kernels instead of the lean ones (a model without optional features otherwise). */
 MJB_API int mjb_state_size(const mjbBatch* b, unsigned int sig);
 MJB_API int mjb_set_state(mjbBatch* b, const double* state /* [nenv][size(sig)] */, unsigned int sig);
@@ -112,7 +113,7 @@ MJB_API int mjb_step_host(mjbBatch* b, const double* ctrl, double* state_out);
 
 /* mj_step for the reference's own mjData objects, one per environment (replaces the per-thread loop
  * `for k: mj_step(m, d[k])`, sample/testspeed.cc:123 / python/mujoco/rollout.cc:85-177): reads time, qpos,
- * qvel, ctrl, qfrc_applied, qacc_warmstart from every d[e], steps the batch once, and writes the new state
+ * qvel, ctrl, qfrc_applied, qacc_warmstart and history from every d[e], steps the batch once, and writes the new state
  * and every fixed-size mjData array the path computes back under the same member names (plus ncon, nefc and
  * the warning counters; arena members - contact, efc_* - stay on the device: use mjb_get_field). */
 struct mjData_;

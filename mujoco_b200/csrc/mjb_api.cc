@@ -162,6 +162,7 @@ mjbBatch* mjb_make_batch(const struct mjModel_* m, int nenv, int nconmax, int nj
   if (const char* ls = getenv("MJB_LANES")) { const int v = atoi(ls); if (v == 16 || v == 32) b.nlane = v; }
   if (H.sz.convex) b.nlane = 32;   // the convex narrow phase is built for the 32-lane mapping only
   if (H.sz.spatial) b.nlane = 32;  // so are spatial tendons
+  if (H.sz.nhistory) b.nlane = 32; // and history buffers
   b.dpitch = ((size_t)b.L.ndbl + 15) / 16 * 16;   // env-major blocks, 128-byte aligned
   b.ipitch = ((size_t)b.L.nint + 31) / 32 * 32;
   size_t nd = b.dpitch * b.stride;
@@ -220,7 +221,7 @@ static int state_segments(const mjbBatch* B, unsigned sig, std::vector<Seg>* seg
   if (sig & ST_QPOS) segs->push_back({L.qpos, S.nq});
   if (sig & ST_QVEL) segs->push_back({L.qvel, S.nv});
   if ((sig & ST_ACT) && S.na) segs->push_back({L.act, S.na});
-  // HISTORY: zero-sized on supported models (nhistory == 0)
+  if ((sig & ST_HISTORY) && S.nhistory) segs->push_back({L.history, S.nhistory});
   if (sig & ST_WARMSTART) segs->push_back({L.qacc_warmstart, S.nv});
   if (sig & ST_CTRL) segs->push_back({L.ctrl, S.nu});
   if (sig & ST_QFRC_APPLIED) segs->push_back({L.qfrc_applied, S.nv});
@@ -508,7 +509,7 @@ int mjb_rollout(mjbBatch* B, int nstep, unsigned int control_spec, const double*
 int mjb_step_host(mjbBatch* B, const double* ctrl, double* state_out) {
   if (!B || !ctrl || !state_out) return fail(MJB_ERR_ARG, "mjb_step_host: bad arguments");
   const int nenv = B->b.nenv, nu = B->hm.dm.sz.nu;
-  const int nstate = 1 + B->hm.dm.sz.nq + B->hm.dm.sz.nv + B->hm.dm.sz.na;
+  const int nstate = 1 + B->hm.dm.sz.nq + B->hm.dm.sz.nv + B->hm.dm.sz.na + B->hm.dm.sz.nhistory;
   if (!B->io_ctrl) {
     B->io_ctrl = (double*)backend::dev_alloc((size_t)nenv * nu * sizeof(double));
     B->io_state = (double*)backend::dev_alloc((size_t)nenv * nstate * sizeof(double));
@@ -525,7 +526,7 @@ int mjb_step_host(mjbBatch* B, const double* ctrl, double* state_out) {
 
 int mjb_rollout_device(mjbBatch* B, int nstep, const double* d_ctrl, double* d_state) {
   if (!B || nstep < 0) return fail(MJB_ERR_ARG, "mjb_rollout_device: bad arguments");
-  const int nstate = 1 + B->hm.dm.sz.nq + B->hm.dm.sz.nv + B->hm.dm.sz.na;
+  const int nstate = 1 + B->hm.dm.sz.nq + B->hm.dm.sz.nv + B->hm.dm.sz.na + B->hm.dm.sz.nhistory;
   // per-step launches (fused step or split step) unless the persistent rollout kernel applies; a persistent kernel
   // whose WARPS drift apart is slower (the instruction working set no longer fits the
   // instruction caches) - mjb_krollout.cu keeps the warps of a CTA in step and lets only the CTAs drift
@@ -557,6 +558,7 @@ static bool find_field(const mjbBatch* B, const char* name, long* off, long* cnt
   MJB_DATA_DBL_FIELDS(X, S)
   MJB_DATA_COLD_FIELDS(X, S)
   MJB_DATA_WRAP_FIELDS(X, S)
+  MJB_DATA_HIST_FIELDS(X, S)
 #undef X
 #define X(fname, count) if (!strcmp(name, #fname)) { *off = L.fname; *cnt = (long)(count); *is_int = true; return true; }
   MJB_DATA_INT_FIELDS(X, S)
@@ -638,6 +640,7 @@ static int bridge_mjdata(mjbBatch* B, mjData* const* d, int nd, BridgeOp op) {
     if (int rc = field_from_host(B, false, B->b.L.name, (cnt), tmp.data())) return rc;            \
   }
   MJB_MJDATA_IN(X)
+  MJB_DATA_HIST_FIELDS(X, S)   // history buffers (allocated only for models with them)
 #undef X
   if (S.neq) {   // mjData.eq_active is a byte array
     tmp.resize((size_t)nenv * S.neq);
@@ -669,6 +672,7 @@ static int bridge_mjdata(mjbBatch* B, mjData* const* d, int nd, BridgeOp op) {
   }
   MJB_MJDATA_OUT(X)
   MJB_DATA_WRAP_FIELDS(X, S)   // spatial tendon paths (allocated only for models with spatial tendons)
+  MJB_DATA_HIST_FIELDS(X, S)   // history buffers
 #undef X
 #define X(name, cnt)                                                                             \
   if ((cnt) > 0) {                                                                               \

@@ -19,8 +19,57 @@
 #include "mjb_collision.h"
 #include "mjb_constraint.h"
 #include "mjb_newton.h"
+#include "mjb_history.h"
 
 namespace mjb {
+
+// history buffers as mj_resetData leaves them (engine_io.c:1404-1454): control samples at -n*dt .. -dt, zero; sensor
+// samples on the same grid, or with an interval at its ticks before the first one rounded up to the timestep grid,
+// the last tick in the user slot (-period for phase 0, else the phase).  Serial (one lane).
+MJB_HD void reset_history(const Env& d) {
+  const DModel& m = d.m;
+  const double dt = m.opt.timestep;
+  FD h = d.history();
+  for (int i = 0; i < m.sz.nu; i++) {
+    const int n = m.actuator_history[2 * i];
+    if (n <= 0) continue;
+    FD buf = h + m.actuator_historyadr[i];
+    buf[0] = 0;
+    buf[1] = n - 1;
+    for (int j = 0; j < n; j++) buf[2 + j] = -(n - j) * dt;
+    for (int j = 0; j < n; j++) buf[2 + n + j] = 0;
+  }
+  for (int i = 0; i < m.sz.nsensor; i++) {
+    const int n = m.sensor_history[2 * i];
+    if (n <= 0) continue;
+    const int dim = m.sensor_dim[i];
+    const double period = m.sensor_interval[2 * i], phase = m.sensor_interval[2 * i + 1];
+    FD buf = h + m.sensor_historyadr[i];
+    buf[0] = (period > 0) ? (phase == 0 ? -period : phase) : -dt;
+    buf[1] = n - 1;
+    if (period > 0) {
+      const double t0 = (phase == 0) ? -period : phase;
+      for (int j = 0; j < n; j++) {
+        const double ct = t0 - (n - 1 - j) * period;
+        buf[2 + j] = ceil(ct / dt) * dt;
+      }
+    } else {
+      for (int j = 0; j < n; j++) buf[2 + j] = -(n - j) * dt;
+    }
+    for (int j = 0; j < n * dim; j++) buf[2 + n + j] = 0;
+  }
+  d.hist_flg()[0] = 0;
+  d.hist_flg()[1] = 0;
+}
+
+// mj_readCtrl (engine_support.c:886-908): a delayed actuator's control at time - delay, read from its buffer
+MJB_HD double read_ctrl(const Env& d, int i) {
+  const DModel& m = d.m;
+  double c;
+  hist_read(d.history() + m.actuator_historyadr[i], m.actuator_history[2 * i], 1, &c, d.time()[0] - m.actuator_delay[i],
+            m.actuator_history[2 * i + 1]);
+  return c;
+}
 
 // mj_resetData for one environment: qpos0, zero velocities/controls/warmstart/time/warnings
 MJB_HD void reset_env(const Env& d, bool clear_warnings) {
@@ -43,6 +92,11 @@ MJB_HD void reset_env(const Env& d, bool clear_warnings) {
   d.time()[0] = 0;
   d.ncon()[0] = 0; d.nefc()[0] = 0; d.ne()[0] = 0; d.nf()[0] = 0; d.nl()[0] = 0; for (int k = 0; k < NISLAND; k++) d.solver_niter()[k] = 0;
   if (clear_warnings) for (int i = 0; i < NWARNING; i++) d.warning()[i] = 0;
+#if defined(MJB_HISTORY_CODE) && defined(__CUDA_ARCH__)
+  if (d.feat & FEAT_HISTORY) reset_history(d);
+#elif defined(MJB_HISTORY_CODE)
+  if (d.m.sz.nhistory) reset_history(d);   // the host emulation is one build for every model (run_env)
+#endif
 }
 
 // scan for NaN / overflow (serial, lane 0 only); on failure raise the warning and (unless
@@ -200,6 +254,7 @@ MJB_HD void fwd_position(const Env& d) {
 }
 
 MJB_HD void object_velocity(const Env& d, int kind, int id, V3& ang, V3& lin);   // defined with the sensors below
+MJB_HD void history_advance(const Env& d);   // defined with the sensors below (FEAT_HISTORY)
 MJB_HD V3 mulmTv(const M3& a, V3 v);
 
 // fluid forces, inertia-box model (mj_fluid / mj_inertiaBoxFluidModel, engine_passive.c:868-903, :1154-1210):
@@ -361,6 +416,9 @@ MJB_HD void tendon_bias(const Env& d) {
 
 MJB_HD void fwd_velocity(const Env& d) {
   const DModel& m = d.m;
+#ifdef MJB_HISTORY_CODE
+  if (d.feat & FEAT_HISTORY) MJB_LANE0 d.hist_flg()[1] = 0;   // mj_fwdVelocity clears flg_subtreevel (engine_forward.c:185)
+#endif
   FD qvel = d.qvel();
   FD tv = d.ten_velocity(), tJ = d.ten_J();
   MJB_PFOR(i, m.sz.ntendon) {
@@ -499,6 +557,9 @@ MJB_HD void fwd_actuation(const Env& d) {
   const bool clamp = !(m.opt.disableflags & DSBL_CLAMPCTRL);
   MJB_PFOR(i, nu) {
     double c = ctrl_in[i];
+#ifdef MJB_HISTORY_CODE
+    if ((d.feat & FEAT_HISTORY) && m.actuator_delay[i] != 0 && m.actuator_history[2 * i] > 0) c = read_ctrl(d, i);
+#endif
     if (clamp && m.actuator_ctrllimited[i]) c = dclip(c, m.actuator_ctrlrange[2 * i], m.actuator_ctrlrange[2 * i + 1]);
     ctrl[i] = c;
   }
@@ -678,6 +739,9 @@ MJB_HD void euler_advance(const Env& d) {
   const double h = m.opt.timestep;
   FD qacc = d.qacc(), qvel = d.qvel();
   FD acc = d.scr_nv();   // acceleration used for the velocity update
+#ifdef MJB_HISTORY_CODE
+  if (d.feat & FEAT_HISTORY) history_advance(d);
+#endif
   if (!m.opt.eulerdamp) {
     MJB_PFOR(i, nv) acc[i] = qacc[i];
     MJB_PSYNC();
@@ -805,6 +869,9 @@ MJB_HD void implicitfast_advance(const Env& d) {
   const bool spring_off = (m.opt.disableflags & DSBL_SPRING) != 0, damper_off = (m.opt.disableflags & DSBL_DAMPER) != 0;
   const bool passive_on = !(spring_off && damper_off) && !damper_off;
   FD tv = d.ten_velocity(), tJ = d.ten_J(), mom = d.actuator_moment(), force = d.actuator_force(), ctrl = d.ctrl();
+#ifdef MJB_HISTORY_CODE
+  if (d.feat & FEAT_HISTORY) history_advance(d);
+#endif
   MJB_PFOR(t, ntendon) {
     tB[t] = passive_on ? -d_xpoly_force(m.tendon_damping_eff[t], m.tendon_dampingpoly_eff + kNPoly * t, kNPoly, tv[t], true) : 0.0;
   }
@@ -1460,15 +1527,89 @@ MJB_HD void contact_sensor(const Env& d, int i, FD out) {
   }
 }
 
-MJB_HD void sensors(const Env& d) {
+// ---- history buffers (FEAT_HISTORY): compute_or_read_sensor (engine_sensor.c:1387-1428) and the lazy inputs ----
+// whether sensor i is computed in this forward pass (else it is read from its buffer)
+MJB_HD bool sensor_computes(const Env& d, int i) {
   const DModel& m = d.m;
-  if (!m.sz.nsensor || (m.opt.disableflags & DSBL_SENSOR)) return;
+  if (m.sensor_history[2 * i] <= 0) return true;
+  if (m.sensor_delay[i] > 0) return false;
+  const double interval = m.sensor_interval[2 * i];
+  if (interval > 0) return d.history()[m.sensor_historyadr[i]] + interval <= d.time()[0];
+  return true;
+}
+// whether mj_advance computes sensor i into a new sample (a delayed sensor whose interval, if any, has elapsed)
+MJB_HD bool sensor_computes_in_advance(const Env& d, int i) {
+  const DModel& m = d.m;
+  if (m.sensor_history[2 * i] <= 0 || !(m.sensor_delay[i] > 0)) return false;
+  const double interval = m.sensor_interval[2 * i];
+  return !(interval > 0) || d.history()[m.sensor_historyadr[i]] + interval <= d.time()[0];
+}
+// mj_rnePostConstraint / mj_subtreeVel run inside the reference's per-sensor computation, once per forward pass (flags
+// flg_rnepost / flg_subtreevel), and only when a sensor that needs them is computed: before the sensors of a forward
+// pass (advance = false) or before the delayed sensors that mj_advance computes (advance = true)
+MJB_HD void lazy_sensor_inputs(const Env& d, bool advance) {
+  const DModel& m = d.m;
+  bool rp = false, sv = false;
+  for (int i = 0; i < m.sz.nsensor; i++) {
+    if (!(advance ? sensor_computes_in_advance(d, i) : sensor_computes(d, i))) continue;
+    const int t = m.sensor_type[i];
+    if (t == SENS_ACCELEROMETER || t == SENS_FORCE || t == SENS_TORQUE || t == SENS_FRAMELINACC || t == SENS_FRAMEANGACC) rp = true;
+    if (t == SENS_SUBTREELINVEL || t == SENS_SUBTREEANGMOM) sv = true;
+  }
+  FI flg = d.hist_flg();
+  rp = rp && m.sz.rnepost && !flg[0];
+  sv = sv && m.sz.subtreevel && !flg[1];
+  MJB_PSYNC();
+  if (rp) rne_post(d);
+  if (sv) subtree_vel(d);
+  MJB_LANE0 { if (rp) flg[0] = 1; if (sv) flg[1] = 1; }
+  MJB_PSYNC();
+}
+// advance (FEAT_HISTORY only): the sensor part of mj_advance instead of the sensors of a forward pass - every sensor
+// with a buffer records a sample at the current time (an interval sensor only once its interval has elapsed, advancing
+// its tick), computed into the new slot when the sensor is delayed, else copied from sensordata
+MJB_HD void sensors(const Env& d, bool advance = false) {
+  const DModel& m = d.m;
+#ifdef MJB_HISTORY_CODE
+  if ((d.feat & FEAT_HISTORY) && !advance) {   // mj_forward clears flg_rnepost whenever it runs the sensors, disabled or not
+    MJB_LANE0 d.hist_flg()[0] = 0;
+    MJB_PSYNC();
+  }
+#endif
+  if (!m.sz.nsensor || ((m.opt.disableflags & DSBL_SENSOR) && !advance)) return;
   const int nefc = d.nefc()[0], nf = d.ne()[0] + d.nf()[0];   // first row after the equality and friction rows
-  FD out = d.sensordata();
+  FD sd = d.sensordata();
   FI etype = d.efc_type(), eid = d.efc_id();
-  if (m.sz.rnepost) rne_post(d);
-  if (m.sz.subtreevel) subtree_vel(d);
+#ifdef MJB_HISTORY_CODE
+  if (d.feat & FEAT_HISTORY) lazy_sensor_inputs(d, advance);
+  else
+#endif
+  {
+    if (m.sz.rnepost) rne_post(d);
+    if (m.sz.subtreevel) subtree_vel(d);
+  }
   MJB_PFOR(i, m.sz.nsensor) {
+    FD out = sd;   // where sensor i's values go (out[sensor_adr ...])
+#ifdef MJB_HISTORY_CODE
+    if (d.feat & FEAT_HISTORY) {
+      const int n = m.sensor_history[2 * i], dim = m.sensor_dim[i], adr = m.sensor_adr[i];
+      FD buf = d.history() + m.sensor_historyadr[i];
+      const double time = d.time()[0];
+      if (!advance) {   // compute_or_read_sensor: a sensor that is not computed now is read at time - delay
+        if (!sensor_computes(d, i)) { hist_read(buf, n, dim, sd + adr, time - m.sensor_delay[i], m.sensor_history[2 * i + 1]); continue; }
+      } else {
+        if (n <= 0) continue;
+        const double interval = m.sensor_interval[2 * i];
+        if (interval > 0) {
+          if (!(buf[0] + interval <= time)) continue;
+          buf[0] += interval;
+        }
+        FD slot = hist_insert(buf, n, dim, time);
+        if (!(m.sensor_delay[i] > 0)) { for (int k = 0; k < dim; k++) slot[k] = sd[adr + k]; continue; }
+        out = slot + (-(long)adr);
+      }
+    }
+#endif
     const int type = m.sensor_type[i], id = m.sensor_objid[i], adr = m.sensor_adr[i], dim = m.sensor_dim[i];
     const int okind = m.sensor_objtype[i], rkind = m.sensor_reftype[i], refid = m.sensor_refid[i];
     double v[4] = {0, 0, 0, 0};
@@ -1647,6 +1788,18 @@ MJB_HD void sensors(const Env& d) {
   MJB_PSYNC();
 }
 
+// the history part of mj_advance (engine_forward.c:1265-1312), at the current time and before the state moves: the
+// control of every actuator with a buffer is recorded, then the sensor samples (sensors, advance = true)
+MJB_HD void history_advance(const Env& d) {
+  const DModel& m = d.m;
+  MJB_PFOR(i, m.sz.nu) {
+    const int n = m.actuator_history[2 * i];
+    if (n > 0) hist_insert(d.history() + m.actuator_historyadr[i], n, 1, d.time()[0])[0] = d.ctrl()[i];
+  }
+  MJB_PSYNC();
+  sensors(d, true);
+}
+
 // explicit Runge-Kutta 4 (mj_RungeKutta, engine_forward.c:1486-1591) split into phases around the
 // forward passes, which are separate launches of the fused kernel:
 //   phase 1..3 (after forward #phase-1): record F[phase-1] = qacc, form X[phase] = X[0] (+) h*dX with the
@@ -1676,6 +1829,16 @@ MJB_HD void rk4_phase(const Env& d, int phase) {
   MJB_PFOR(i, nv) F[(phase - 1) * nv + i] = qacc[i];
   MJB_PFOR(i, na) Fa[(phase - 1) * na + i] = act_dot[i];
   MJB_PSYNC();
+#ifdef MJB_HISTORY_CODE
+  if ((d.feat & FEAT_HISTORY) && phase == 4) {   // mj_advance runs on the restored X[0] and time, stage-4 derived quantities
+    MJB_PFOR(i, nq) qpos[i] = x0q[i];
+    MJB_PFOR(i, nv) qvel[i] = x0v[i];
+    MJB_PFOR(i, na) act[i] = x0a[i];
+    MJB_LANE0 d.time()[0] = t0[0];
+    MJB_PSYNC();
+    history_advance(d);
+  }
+#endif
   auto Xv = [&](int j, int i) { return j == 0 ? x0v[i] : xv[(j - 1) * nv + i]; };
   if (phase < 4) {
     MJB_PFOR(i, nv) {

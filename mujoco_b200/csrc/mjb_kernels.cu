@@ -52,6 +52,14 @@ __global__ void k_reset(DModel m, Batch b) {
   reset_env(d, true);
 }
 
+// history buffers as mj_resetData leaves them (models with history buffers, after k_reset)
+__global__ void k_reset_history(DModel m, Batch b) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= b.nenv) return;
+  Env d(m, b, e);
+  reset_history(d);
+}
+
 __global__ void k_set_control(DModel m, Batch b, const double* control, int nstep, int t, unsigned spec, int ncontrol, int skip_warned) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= b.nenv) return;
@@ -78,6 +86,18 @@ __global__ void k_get_state(DModel m, Batch b, double* state, int nstep, int t, 
   Env d(m, b, e);
   const int nq = m.sz.nq, nv = m.sz.nv;
   const double v = (k == 0) ? d.time()[0] : (k <= nq) ? d.qpos()[k - 1] : (k <= nq + nv) ? d.qvel()[k - 1 - nq] : d.act()[k - 1 - nq - nv];
+  state[((size_t)e * nstep + t) * nstate + k] = v;
+}
+
+// k_get_state for models with history buffers: the state row ends with the history segment
+__global__ void k_get_state_history(DModel m, Batch b, double* state, int nstep, int t, int nstate) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long)b.nenv * nstate) return;
+  const int e = (int)(idx / nstate), k = (int)(idx - (long)e * nstate);
+  Env d(m, b, e);
+  const int nq = m.sz.nq, nv = m.sz.nv, na = m.sz.na;
+  const double v = (k == 0) ? d.time()[0] : (k <= nq) ? d.qpos()[k - 1] : (k <= nq + nv) ? d.qvel()[k - 1 - nq]
+                 : (k <= nq + nv + na) ? d.act()[k - 1 - nq - nv] : d.history()[k - 1 - nq - nv - na];
   state[((size_t)e * nstep + t) * nstate + k] = v;
 }
 
@@ -208,10 +228,10 @@ int launch_fill_zero(const Batch& b, int is_int, long off, long cnt, void* s) {
 }
 
 // lean kernels (FEAT = 0) when the model needs none of the optional pipeline parts (FEAT_*); a model with convex
-// collision pairs or spatial tendons is never lean, since only the FEAT_CONVEX / FEAT_SPATIAL instantiations carry
-// their code
+// collision pairs, spatial tendons or history buffers is never lean, since only the FEAT_CONVEX / FEAT_SPATIAL /
+// FEAT_HISTORY instantiations carry their code
 static bool lean_model(const DModel& dm, const Batch& b) {
-  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc && !dm.sz.convex && !dm.sz.spatial;
+  return dm.sz.nsensor == 0 && dm.sz.neq == 0 && dm.sz.ntree == 1 && dm.opt.integrator != INT_IMPLICITFAST && !dm.sz.actfeat && !dm.sz.colbox && !dm.sz.epot && !dm.sz.ekin && !b.xfrc && !dm.sz.convex && !dm.sz.spatial && !dm.sz.nhistory;
 }
 
 // split step: position + velocity | PGS (4 lanes per environment, mjb_pgs4.cu) | finish + integrate | redo
@@ -220,7 +240,7 @@ bool split_step_available(const DModel& dm, const Batch& b) {
   static int want = -1;
   if (want < 0) { const char* s = getenv("MJB_SPLIT"); want = s ? atoi(s) : 1; }
   const bool islands = dm.sz.ntree > 1 && !(dm.opt.disableflags & DSBL_ISLAND);
-  return want && b.warp_per_env && b.nlane == 32 && !dm.sz.convex && !dm.sz.spatial && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
+  return want && b.warp_per_env && b.nlane == 32 && !dm.sz.convex && !dm.sz.spatial && !dm.sz.nhistory && dm.opt.solver == SOL_PGS && !islands && dm.opt.noslip_iterations <= 0 &&
          (dm.opt.integrator == INT_EULER || dm.opt.integrator == INT_IMPLICITFAST);
 }
 int launch_split_step(const DModel& dm, const Batch& b, int first, int later, void* s, void* stagger) {
@@ -300,7 +320,9 @@ int profile_split_step(const DModel& dm, const Batch& b, void* s, float* ms) {
 }
 
 int launch_stages(const DModel& dm, const Batch& b, int mask, int flags, void* s) {
-  if (dm.sz.spatial) {   // spatial tendons: only these instantiations carry the tendon paths (32 lanes or one lane per env)
+  if (dm.sz.nhistory) {   // history buffers: only these instantiations carry them (32 lanes or one lane per env)
+    if (b.warp_per_env) launch_kstep_history32(dm, b, mask, flags, s); else launch_kstep_lane_history(dm, b, mask, flags, s);
+  } else if (dm.sz.spatial) {   // spatial tendons: only these instantiations carry the tendon paths (32 lanes or one lane per env)
     if (b.warp_per_env) launch_kstep_spatial32(dm, b, mask, flags, s); else launch_kstep_lane_spatial(dm, b, mask, flags, s);
   } else if (dm.sz.convex) {   // convex collision pairs: only these instantiations carry GJK / EPA (32 lanes or one lane per env)
     if (b.warp_per_env) launch_kstep_convex32(dm, b, mask, flags, s); else launch_kstep_lane_convex(dm, b, mask, flags, s);
@@ -327,13 +349,15 @@ int launch_get_sensor(const DModel& dm, const Batch& b, double* sens, int nstep,
   return 0;
 }
 int launch_rk4(const DModel& dm, const Batch& b, int phase, int flags, void* s) {
-  k_rk4<<<(b.nenv + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, (cudaStream_t)s>>>(dm, b, phase, flags);
+  if (dm.sz.nhistory) launch_rk4_history(dm, b, phase, flags, s);   // the sensor code of mj_advance (mjb_kstep_history32.cu)
+  else k_rk4<<<(b.nenv + kWarpsPerCta - 1) / kWarpsPerCta, 32 * kWarpsPerCta, 0, (cudaStream_t)s>>>(dm, b, phase, flags);
   g_launches++;
   CK(cudaPeekAtLastError(), "rk4 kernel launch");
   return 0;
 }
 int launch_reset(const DModel& dm, const Batch& b, void* s) {
   k_reset<<<nblocks(b, 128), 128, 0, (cudaStream_t)s>>>(dm, b);
+  if (dm.sz.nhistory) k_reset_history<<<nblocks(b, 128), 128, 0, (cudaStream_t)s>>>(dm, b);
   g_launches++;
   CK(cudaPeekAtLastError(), "k_reset launch");
   return 0;
@@ -350,7 +374,8 @@ int launch_set_control(const DModel& dm, const Batch& b, const double* control, 
   return 0;
 }
 int launch_get_state(const DModel& dm, const Batch& b, double* state, int nstep, int t, int nstate, void* s) {
-  k_get_state<<<(unsigned)(((long)b.nenv * nstate + 255) / 256), 256, 0, (cudaStream_t)s>>>(dm, b, state, nstep, t, nstate);
+  if (dm.sz.nhistory) k_get_state_history<<<(unsigned)(((long)b.nenv * nstate + 255) / 256), 256, 0, (cudaStream_t)s>>>(dm, b, state, nstep, t, nstate);
+  else k_get_state<<<(unsigned)(((long)b.nenv * nstate + 255) / 256), 256, 0, (cudaStream_t)s>>>(dm, b, state, nstep, t, nstate);
   g_launches++;
   CK(cudaPeekAtLastError(), "k_get_state launch");
   return 0;

@@ -22,6 +22,11 @@ void launch_kstep_lane_convex(const DModel& dm, const Batch& b, int mask, int fl
 // validation mapping (mjb_kstep_spatial32.cu)
 void launch_kstep_spatial32(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
 void launch_kstep_lane_spatial(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
+// history buffers (FEAT_ALL | FEAT_HISTORY, solver chosen at run time): fused 32-lane kernel, the lane-per-env
+// validation mapping and the Runge-Kutta phase kernel, whose last phase records samples (mjb_kstep_history32.cu)
+void launch_kstep_history32(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
+void launch_kstep_lane_history(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
+void launch_rk4_history(const DModel& dm, const Batch& b, int phase, int flags, void* stream);
 // lean instantiations (FEAT = 0): models without sensors, equalities, several trees or implicitfast
 void launch_kstep_pgs32_lean(const DModel& dm, const Batch& b, int mask, int flags, void* stream);
 void launch_kstep_newton32_lean(const DModel& dm, const Batch& b, int mask, int flags, void* stream);

@@ -370,14 +370,14 @@ int check_model(const mjModel* m) {
     int code, okind, rkind;
     if (!sensor_code(m, i, &code, &okind, &rkind))
       FAIL("sensor %d: type %d / object type %d is outside the supported set", i, (int)m->sensor_type[i], (int)m->sensor_objtype[i]);
-    if (m->sensor_history[2 * i] > 0 || m->sensor_delay[i] > 0 || m->sensor_interval[2 * i] > 0) FAIL("sensor %d: history / delay / interval", i);
   }
   for (int i = 0; i < m->npair; i++) {
     // solreffriction only shapes the friction rows of ELLIPTIC cones (mj_makeImpedance); pyramidal rows take solref
     if ((m->pair_solreffriction[mjNREF * i] || m->pair_solreffriction[mjNREF * i + 1]) && m->opt.cone != mjCONE_PYRAMIDAL) FAIL("contact pair %d: solreffriction", i);
     if (m->pair_adhesion[i] != 0) FAIL("contact pair %d: adhesion", i);
   }
-  if (m->nhistory) FAIL("history buffers / delays");
+  // mj_resetData places the history samples on the timestep grid and refuses a non-positive timestep (engine_io.c)
+  if (m->nhistory && !(m->opt.timestep > 0)) FAIL("history buffers with a timestep <= 0");
   if (m->flg_surfacevel) FAIL("geom surface velocity");
   if (m->opt.cone != mjCONE_PYRAMIDAL) FAIL("elliptic friction cones");
   if (m->opt.integrator == mjINT_IMPLICIT) FAIL("the fully implicit integrator (RNE velocity derivatives, sparse LU)");
@@ -431,7 +431,6 @@ int check_model(const mjModel* m) {
     if (gt == mjGAIN_MUSCLE && m->opt.integrator == mjINT_IMPLICITFAST) FAIL("actuator %d: muscle gain with implicitfast (velocity derivative of the FLV curve)", i);
     if (m->actuator_ctrlnum[i] != 1 || m->actuator_outnum[i] != 1 || m->actuator_ctrladr[i] != i || m->actuator_outadr[i] != i)
       FAIL("actuator %d: non-scalar control block", i);
-    if (m->actuator_delay[i] != 0) FAIL("actuator %d: delay", i);
     if (m->actuator_plugin[i] >= 0) FAIL("actuator %d: plugin", i);
     if (m->opt.disableactuator & (1 << m->actuator_group[i])) FAIL("disabled actuator groups");
   }
@@ -630,6 +629,18 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
     }
     B.addI(&D.tendon_slotadr, slot.data(), m->ntendon);
     B.addI(&D.body_simple, m->body_simple, m->nbody);
+  }
+  {   // history buffers (mjData.history): [nsample, interp] and the buffer address of each actuator and sensor, the
+      // delays, and the sensors' [period, phase]
+    S.nhistory = (int)m->nhistory;
+    S.histflg = m->nhistory > 0 ? 1 : 0;
+    B.addI(&D.actuator_history, m->actuator_history, 2 * m->nu);
+    B.addI(&D.actuator_historyadr, m->actuator_historyadr, m->nu);
+    B.addI(&D.sensor_history, m->sensor_history, 2 * m->nsensor);
+    B.addI(&D.sensor_historyadr, m->sensor_historyadr, m->nsensor);
+    B.addD(&D.actuator_delay, m->actuator_delay, m->nu);
+    B.addD(&D.sensor_delay, m->sensor_delay, m->nsensor);
+    B.addD(&D.sensor_interval, m->sensor_interval, 2 * m->nsensor);
   }
   {
     std::vector<int> trn(m->nu);
@@ -977,6 +988,14 @@ int build_host_model(const mjModel* m, int nconmax, int njmax, HostModel* out) {
     }
   }
   S.npair = (int)pg1.size();
+  if (S.nhistory && S.spatial) {
+    set_error("unsupported: history buffers (delays) together with spatial tendons: no kernel carries both");
+    return -2;
+  }
+  if (S.nhistory && S.convex) {
+    set_error("unsupported: history buffers (delays) together with convex (GJK / EPA) collision pairs: no kernel carries both");
+    return -2;
+  }
   if (S.spatial && S.convex) {
     set_error("unsupported: spatial tendons together with convex (GJK / EPA) collision pairs: no kernel carries both");
     return -2;

@@ -105,6 +105,7 @@ MJB_HD void run_env(const DModel& m, const Batch& b, int e, int mask, int flags,
   // only in mjb_kstep_spatial32.cu).
   if (m.sz.convex) feat |= FEAT_CONVEX;
   if (m.sz.spatial) feat |= FEAT_SPATIAL;
+  if (m.sz.nhistory) feat |= FEAT_HISTORY;
 #endif
   d.sm = sm; d.smcap = smcap; d.mask = lanes; d.feat = feat;
   d.solver = solver < 0 ? m.opt.solver : solver;
@@ -122,9 +123,14 @@ MJB_HD void run_env(const DModel& m, const Batch& b, int e, int mask, int flags,
   else run_stage_mask(d, mask, flags);
 }
 
-// one phase of the Runge-Kutta step (between forward launches)
-MJB_HD void run_rk4(const DModel& m, const Batch& b, int e, int phase, int flags, int lane, int nlane) {
+// one phase of the Runge-Kutta step (between forward launches); models with history buffers take the FEAT_HISTORY
+// instantiation (mjb_kstep_history32.cu), whose last phase runs the history part of mj_advance
+MJB_HD void run_rk4(const DModel& m, const Batch& b, int e, int phase, int flags, int lane, int nlane, int feat = FEAT_ALL) {
   Env d(m, b, e, lane, nlane);
+#if !defined(__CUDA_ARCH__)
+  if (m.sz.nhistory) feat |= FEAT_HISTORY;
+#endif
+  d.feat = feat;
   d.solver = m.opt.solver;
   if (!step_enabled(d, flags)) return;
   rk4_phase(d, phase);
@@ -147,7 +153,7 @@ MJB_HD void run_set_control(const DModel& m, const Batch& b, int e, const double
   if (spec & (1u << 11)) { FD q = d.mocap_quat(); for (int i = 0; i < 4 * m.sz.nmocap; i++) q[i] = src[k++]; }
 }
 
-// state [nenv][nstep][nstate] = (time, qpos, qvel, act)  (mjSTATE_FULLPHYSICS)
+// state [nenv][nstep][nstate] = (time, qpos, qvel, act, history)  (mjSTATE_FULLPHYSICS)
 MJB_HD void run_get_state(const DModel& m, const Batch& b, int e, double* state, int nstep, int t, int nstate) {
   Env d(m, b, e);
   double* dst = state + ((size_t)e * nstep + t) * nstate;
@@ -157,6 +163,7 @@ MJB_HD void run_get_state(const DModel& m, const Batch& b, int e, double* state,
   for (int i = 0; i < m.sz.nq; i++) dst[k++] = qp[i];
   for (int i = 0; i < m.sz.nv; i++) dst[k++] = qv[i];
   for (int i = 0; i < m.sz.na; i++) dst[k++] = d.act()[i];
+  for (int i = 0; i < m.sz.nhistory; i++) dst[k++] = d.history()[i];
 }
 
 // sensordata [nenv][nstep][nsensordata]; a warned env repeats its last values (the reference pads likewise)
@@ -183,6 +190,7 @@ MJB_HD void run_get_state_native(const DModel& m, const Batch& b, int e, double*
   for (int i = 0; i < m.sz.nq; i++) dst[(size_t)(k++) * b.stride] = qp[i];
   for (int i = 0; i < m.sz.nv; i++) dst[(size_t)(k++) * b.stride] = qv[i];
   for (int i = 0; i < m.sz.na; i++) dst[(size_t)(k++) * b.stride] = d.act()[i];
+  for (int i = 0; i < m.sz.nhistory; i++) dst[(size_t)(k++) * b.stride] = d.history()[i];
 }
 
 // dense [nenv][cnt] <-> field of either layout; idx enumerates (env, elem)

@@ -32,11 +32,13 @@ enum { WARN_INERTIA = 0, WARN_CONTACTFULL = 1, WARN_CNSTRFULL = 2, WARN_BADQPOS 
        WARN_BADQVEL = 4, WARN_BADQACC = 5, WARN_BADCTRL = 6, WARN_VGEOMFULL = 7, NWARNING = 8 };
 enum { NISLAND = 20 };
 enum { FEAT_SENSOR = 1, FEAT_EQUALITY = 2, FEAT_ISLAND = 4, FEAT_IMPLICITFAST = 8, FEAT_ACT = 16, FEAT_COLBOX = 32, FEAT_ALL = 63,
-       FEAT_CONVEX = 64, FEAT_SPATIAL = 128 };   // FEAT_COLBOX: cylinder / box colliders (up to 8 contacts per pair)   // FEAT_ACT: stateful actuators (act), tendon transmissions, muscles
+       FEAT_CONVEX = 64, FEAT_SPATIAL = 128, FEAT_HISTORY = 256 };   // FEAT_COLBOX: cylinder / box colliders (up to 8 contacts per pair)   // FEAT_ACT: stateful actuators (act), tendon transmissions, muscles
 // FEAT_CONVEX: GJK / EPA narrow phase (mjb_convex.h).  Outside FEAT_ALL on purpose: only the convex instantiations
 // carry its code and its polytope scratch, every other kernel compiles exactly as without it.
 // FEAT_SPATIAL: spatial tendons (site paths, sphere / cylinder wrapping, pulleys) and their tendon-armature bias.
 // Outside FEAT_ALL for the same reason: only the spatial instantiations (mjb_kstep_spatial32.cu) carry it.
+// FEAT_HISTORY: actuator and sensor history buffers (delayed controls, delayed / sampled sensors, mjb_history.h).
+// Outside FEAT_ALL as well: only the history instantiations (mjb_kstep_history32.cu) carry it.
 enum { WRAP_NONE = 0, WRAP_JOINT = 1, WRAP_PULLEY = 2, WRAP_SITE = 3, WRAP_SPHERE = 4, WRAP_CYLINDER = 5 };   // mjtWrap (mjtype.h:220-227)
 enum { EQ_JOINT = 0, EQ_TENDON = 1, EQ_CONNECT = 2, EQ_WELD = 3 };   // supported equality kinds (body semantics)
 constexpr int kNEqData = 11;            // eq_data values per equality (mjNEQDATA): polycoef / anchors, relpose, torquescale
@@ -93,6 +95,8 @@ struct Sizes {
   int ccdslots;  // polytope slots per environment (ccd_poly), 0 without GJK candidates
   int ccdslot;   // doubles per polytope slot (ccd_slot_doubles(ccd_iterations))
   int spatial;   // 1 when a tendon is spatial (FEAT_SPATIAL code paths; the wrap fields of the batch are allocated then)
+  int nhistory;  // doubles of the actuator and sensor history buffers (FEAT_HISTORY code paths when > 0)
+  int histflg;   // 1 when nhistory > 0 (the lazy-evaluation flags of the batch are allocated then)
 };
 
 struct Options {
@@ -132,7 +136,8 @@ struct Options {
   X(sensor_type) X(sensor_cutmode) X(sensor_objtype) X(sensor_objid) X(sensor_reftype) X(sensor_refid)   \
   X(sensor_dim) X(sensor_adr) X(sensor_intprm0) X(sensor_intprm1) X(sensor_objraw) X(sensor_refraw) X(geom_rayskip) X(site_bodyid) X(site_sameframe)                               \
   X(eq_kind) X(eq_obj1id) X(eq_obj2id) X(eq_active0)                                          \
-  X(body_simple) X(tendon_slotadr)
+  X(body_simple) X(tendon_slotadr)                                                            \
+  X(actuator_history) X(actuator_historyadr) X(sensor_history) X(sensor_historyadr)
 
 #define MJB_MODEL_DBL_FIELDS(X)                                                             \
   X(qpos0) X(qpos_spring) X(body_pos) X(body_quat) X(body_ipos) X(body_iquat) X(body_mass)   \
@@ -149,7 +154,8 @@ struct Options {
   X(actuator_forcerange) X(actuator_dynprm) X(actuator_actrange) X(actuator_lengthrange) X(actuator_acc0) \
   X(site_size) X(body_gravcomp) X(actuator_gear6) X(actuator_cranklength) X(actuator_wrapperiod) X(tendon_frictionloss) X(tendon_solref_fri) X(tendon_solimp_fri) X(tendon_actfrcrange)      \
   X(pair_margin) X(pair_includemargin) X(pair_solref) X(pair_solimp) X(pair_friction) X(sensor_cutoff) X(site_pos) X(site_quat)            \
-  X(eq_data) X(eq_solref) X(eq_solimp) X(tendon_length0)
+  X(eq_data) X(eq_solref) X(eq_solimp) X(tendon_length0)                                      \
+  X(actuator_delay) X(sensor_delay) X(sensor_interval)
 
 struct DModel {
   Sizes sz;
@@ -208,6 +214,11 @@ struct DModel {
 #define MJB_DATA_WRAP_INT_FIELDS(X, S)                                                        \
   X(ten_wrapadr, S.ntendon * S.spatial) X(ten_wrapnum, S.ntendon * S.spatial) X(wrap_obj, 2 * S.nwrap * S.spatial)
 
+// history buffers (empty for models without them): mjData.history, and the lazy-evaluation flags of
+// mj_rnePostConstraint / mj_subtreeVel (mjData.flg_rnepost, flg_subtreevel).  Laid out after every other field.
+#define MJB_DATA_HIST_FIELDS(X, S) X(history, S.nhistory)
+#define MJB_DATA_HIST_INT_FIELDS(X, S) X(hist_flg, 2 * S.histflg)
+
 // ints (all hot)
 #define MJB_DATA_INT_FIELDS(X, S)                                                            \
   X(ncon, 1) X(nefc, 1) X(ne, 1) X(nf, 1) X(nl, 1) X(solver_niter, NISLAND) X(step_skip, 1) X(warning, NWARNING)  \
@@ -230,6 +241,8 @@ struct Layout {
   MJB_DATA_CCD_FIELDS(X, _)
   MJB_DATA_WRAP_FIELDS(X, _)
   MJB_DATA_WRAP_INT_FIELDS(X, _)
+  MJB_DATA_HIST_FIELDS(X, _)
+  MJB_DATA_HIST_INT_FIELDS(X, _)
 #undef X
 };
 
@@ -243,10 +256,12 @@ inline Layout make_layout(const Sizes& S) {
   MJB_DATA_COLD_FIELDS(X, S)
   MJB_DATA_CCD_FIELDS(X, S)
   MJB_DATA_WRAP_FIELDS(X, S)
+  MJB_DATA_HIST_FIELDS(X, S)
   L.ndbl = o;
   o = 0;
   MJB_DATA_INT_FIELDS(X, S)
   MJB_DATA_WRAP_INT_FIELDS(X, S)
+  MJB_DATA_HIST_INT_FIELDS(X, S)
   L.nint = o;
 #undef X
   return L;
@@ -312,10 +327,12 @@ struct Env {
   MJB_DATA_COLD_FIELDS(X, _)
   MJB_DATA_CCD_FIELDS(X, _)
   MJB_DATA_WRAP_FIELDS(X, _)
+  MJB_DATA_HIST_FIELDS(X, _)
 #undef X
 #define X(name, cnt) MJB_HD FI name() const { return FI{hi + b.L.name}; }
   MJB_DATA_INT_FIELDS(X, _)
   MJB_DATA_WRAP_INT_FIELDS(X, _)
+  MJB_DATA_HIST_INT_FIELDS(X, _)
 #undef X
   // barrier + memory ordering between the lanes that share this environment
   MJB_HD void sync() const {
